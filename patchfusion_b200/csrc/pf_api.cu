@@ -342,19 +342,27 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
       }
     }
   }
-  // The kernels hold the 128 x block_n fp32 accumulator tile in the registers of two consumer warpgroups; half tiles of
-  // up to 64 columns leave the epilogue room without spilling.  A 192- or 256-column choice (the packed weights stay
-  // padded for it) therefore runs as two n-tiles of half the width, unless a fused trailing layer needs the whole row
-  // in one tile.
-  if (u->block_n == 0 && bn > 128 && bn % 64 == 0 && !u->w2) bn /= 2;
-  d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
-  u->block_n = bn; u->n_tiles = d.n_tiles;
-  d.M = u->M; d.NB = u->NB; d.H = u->H; d.W = u->W;
-  CUtensorMap tmA[3], tmB;
   // 3x3 convs go through the halo-tile kernel (one A fetch per 64-channel chunk instead of nine) unless the caller
   // pins a tile shape or PF_B200_NO_HALO is set.
   static const bool no_halo = getenv("PF_B200_NO_HALO") != nullptr;
   const bool halo = u->a_mode == 1 && u->taps == 9 && u->bh == 0 && u->bw == 0 && !no_halo;
+  if (halo && u->block_n == 0) {
+    // The halo kernel is compiled for block_n 32, 64, 128 and 192 (a warpgroup's 64 x block_n fp32 accumulator in
+    // registers): the widest that divides the packed panel's rows, so the last n-tile reads zero-packed rows only.  A
+    // fused trailing layer wider than that is refused below (it needs the whole row in one n-tile).
+    const int n_pad = (u->N + bn - 1) / bn * bn;
+    bn = n_pad % 192 == 0 ? 192 : (n_pad % 128 == 0 ? 128 : (n_pad % 64 == 0 ? 64 : 32));
+  } else if (!halo && u->block_n == 0 && bn > 128 && bn % 64 == 0 && !u->w2) {
+    // pf_gemm_kernel holds the 128 x block_n fp32 accumulator tile in the registers of two consumer warpgroups; half
+    // tiles of up to 64 columns leave the epilogue room without spilling.  A 192- or 256-column choice (the packed
+    // weights stay padded for it) therefore runs as two n-tiles of half the width, unless a fused trailing layer needs
+    // the whole row in one tile.
+    bn /= 2;
+  }
+  d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
+  u->block_n = bn; u->n_tiles = d.n_tiles;
+  d.M = u->M; d.NB = u->NB; d.H = u->H; d.W = u->W;
+  CUtensorMap tmA[3], tmB;
   d.halo = halo ? 1 : 0;
   bool any_rs = false;
   for (int s = 0; s < u->num_src; ++s) {

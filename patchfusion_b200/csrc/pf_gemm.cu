@@ -15,7 +15,8 @@
 // rows, so there is no im2col buffer and no halo code.  Weights are pre-packed K-major [N, Ktot] with every
 // (source, tap) segment padded to a multiple of 64 channels, matching the producer's enumeration order.
 //
-// Warp roles: warps 0-7 = two consumer warpgroups.  Warpgroup h computes columns [h * block_n / 2,
+// Warp roles (pf_gemm_kernel; the halo kernel below splits its tile by rows instead): warps 0-7 = two consumer
+// warpgroups.  Warpgroup h computes columns [h * block_n / 2,
 // (h + 1) * block_n / 2) of the 128-row tile with wgmma (A fragments loaded by ldmatrix from the swizzled TMA tile, B
 // read by the tensor core from shared memory); warp w of a warpgroup owns tile rows 32 (w & 3) .. 32 (w & 3) + 31,
 // fed to the instruction as two 16-row halves, so after the mainloop every accumulator row lives in one warp.  The
@@ -25,8 +26,6 @@
 // the fused-tail / residual / pixel-shuffle / V^T variants.  The last warp is the TMA producer; the halo kernel has
 // two more warps before it, the operand producers of its optional fused bilinear resample (idle otherwise).  While the consumers drain a tile, the
 // producer already fills the operand ring for the next one.
-#include <stdlib.h>
-
 #include "pf_common.cuh"
 #include "pf_kernels.h"
 
@@ -35,10 +34,10 @@ namespace pf {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KiB
-constexpr int kEpiWarps = 8;                       // consumer warps: two warpgroups, one per half of the N tile
+constexpr int kEpiWarps = 8;                       // consumer warps: two warpgroups
 // pf_gemm_kernel: consumers + one TMA producer warp; pf_conv3_halo_kernel: + two resample producer warps before it.
-// A consumer thread holds 2 x 64 fp32 accumulators plus 32 A-fragment registers: no idle warps, so that the
-// per-thread register budget (65536 / threads) stays above ~180.
+// A consumer thread holds up to 2 x 64 (pf_gemm_kernel) or 96 (halo kernel) fp32 accumulators plus 32 A-fragment
+// registers: no idle warps, so that the per-thread register budget (65536 / threads, capped at 168) stays large.
 constexpr int kGemmThreads = (kEpiWarps + 1) * 32;
 constexpr int kHaloThreads = (kEpiWarps + 3) * 32;
 constexpr int kRsWarp0 = kEpiWarps;                         // halo kernel: warps 8, 9 = resample producers
@@ -52,7 +51,6 @@ struct GemmKernelParams {
   int stages;
   int total_tiles;
   int k_steps;  // per tile
-  int kc;       // halo kernel: taps per weight stage (1, 3 or 9)
 };
 
 
@@ -308,17 +306,22 @@ __device__ __forceinline__ void acc_stage_k(int k, const float (&a0)[S], const f
   else if (k == 2) acc_stage<S <= 32 ? 1 : 2>(a0, a1, buf, lane);
   else acc_stage<S <= 32 ? 1 : 3>(a0, a1, buf, lane);
 }
+// word j of this thread's staged row: rowp[j ^ s] (rowp = the 32-word row, s = its swizzle)
+template <int W>
+__device__ __forceinline__ void acc_read_row(const float* rowp, int s, uint32_t (&v)[W]) {
+#pragma unroll
+  for (int j = 0; j < W; ++j) v[j] = __float_as_uint(rowp[j ^ s]);
+}
 template <int W>
 __device__ __forceinline__ void acc_read(const float* buf, int lane, uint32_t (&v)[W]) {
-  const int s = xpose_swz(lane);
-#pragma unroll
-  for (int j = 0; j < W; ++j) v[j] = __float_as_uint(buf[lane * 32 + (j ^ s)]);
+  acc_read_row<W>(buf + lane * 32, xpose_swz(lane), v);
 }
 
 
-// one W-column chunk starting at accumulator column cb of this thread's row (staged in buf by the caller)
+// one W-column chunk starting at accumulator column cb of this thread's row (staged by the caller; read through
+// acc_read_row(rowp, sw))
 template <int W, int TAILN>
-__device__ __forceinline__ void epilogue_cols(const GemmDesc& d, const float* buf, int lane, int cb, const TileCoord& c,
+__device__ __forceinline__ void epilogue_cols(const GemmDesc& d, const float* rowp, int sw, int cb, const TileCoord& c,
                                               int ocol0, long long orow, bool row_ok, float (&y2)[kMaxTail]) {
   const int ncol = c.n0 + cb;            // global N index of v[0] (selects the V^T path)
   const int lcol = ocol0 + cb;           // logical output channel of v[0] (bias / gamma / residual index)
@@ -334,7 +337,7 @@ __device__ __forceinline__ void epilogue_cols(const GemmDesc& d, const float* bu
     for (int j = 0; j < (TAILN == 0 ? W / 8 : 1); ++j) ld_global_256(xp + 8 * j, xpre[j]);
   }
   uint32_t v[W];
-  acc_read<W>(buf, lane, v);
+  acc_read_row<W>(rowp, sw, v);
   float f[W];
 #pragma unroll
   for (int j = 0; j < W; ++j) f[j] = __uint_as_float(v[j]);
@@ -348,11 +351,13 @@ __device__ __forceinline__ void epilogue_row(const GemmDesc& d, const float (&a0
                                              int lane, int half, const TileCoord& c, int ocol0, long long orow, bool row_ok,
                                              float (&y2)[kMaxTail]) {
   const int nh = d.block_n >> 1;
+  const float* rowp = buf + lane * 32;
+  const int sw = xpose_swz(lane);
   for (int k = 0; 32 * k < nh; ++k) {
     acc_stage_k(k, a0, a1, buf, lane);
     __syncwarp();
-    if (32 * k + 32 <= nh) epilogue_cols<32, TAILN>(d, buf, lane, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
-    else epilogue_cols<16, TAILN>(d, buf, lane, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
+    if (32 * k + 32 <= nh) epilogue_cols<32, TAILN>(d, rowp, sw, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
+    else epilogue_cols<16, TAILN>(d, rowp, sw, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
     __syncwarp();
   }
 }
@@ -525,6 +530,21 @@ __device__ __forceinline__ TileIter make_iter(const GemmDesc& d, int total_tiles
   return it;
 }
 
+// fused trailing layer output of one row: fp32 [rows, out3_ld], bias + activation
+__device__ __forceinline__ void tail_store(const GemmDesc& d, long long orow, const float (&y2)[kMaxTail]) {
+  float* op = d.out3 + orow * d.out3_ld;
+#pragma unroll
+  for (int i = 0; i < kMaxTail; ++i) {
+    if (i < d.n2) {
+      float v2 = y2[i] + (d.b2 != nullptr ? __ldg(d.b2 + i) : 0.f);
+      if (d.act2 == PF_ACT_RELU) v2 = fmaxf(v2, 0.f);
+      else if (d.act2 == PF_ACT_SOFTPLUS) v2 = softplus(v2);
+      else if (d.act2 == PF_ACT_GELU) v2 = gelu_erf(v2);
+      op[i] = v2;
+    }
+  }
+}
+
 // Epilogue of one tile by consumer warp `warp` (rows 32 (warp & 3) + lane, the columns of warpgroup warp >> 2).
 template <int S>
 __device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord& c, const float (&a0)[S],
@@ -592,20 +612,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord
     }
     asm volatile("bar.sync %0, 64;" ::"r"(q + 1) : "memory");
   }
-  if (d.w2 != nullptr && row_ok && half == 0) {
-    // trailing layer output: fp32 [rows, out3_ld], bias + activation
-    float* op = d.out3 + orow * d.out3_ld;
-#pragma unroll
-    for (int i = 0; i < kMaxTail; ++i) {
-      if (i < d.n2) {
-        float v2 = y2[i] + (d.b2 != nullptr ? __ldg(d.b2 + i) : 0.f);
-        if (d.act2 == PF_ACT_RELU) v2 = fmaxf(v2, 0.f);
-        else if (d.act2 == PF_ACT_SOFTPLUS) v2 = softplus(v2);
-        else if (d.act2 == PF_ACT_GELU) v2 = gelu_erf(v2);
-        op[i] = v2;
-      }
-    }
-  }
+  if (d.w2 != nullptr && row_ok && half == 0) tail_store(d, orow, y2);
 }
 
 // Columns warpgroup `half` issues for tile t: its share of tile_n_eff (a multiple of 16, possibly 0).
@@ -781,11 +788,32 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
 // output tile (23 KB) and all nine taps are issued from it: for tap (dy,dx) accumulator row r = 8 yy + xx reads halo
 // pixel (yy + dy) * 10 + xx + dx, so the consumers' ldmatrix row addresses simply shift per tap (the 128B-swizzle XOR
 // is a function of the shared-memory address bits, so shifted rows of a TMA-written tile are read the same way).
-// A traffic from L2 drops 6.3x; the weights stream per (chunk, tap) as before.  Warp roles are those of pf_gemm_kernel.
+// A traffic from L2 drops 6.3x; the weights stream per (chunk, tap) as before.
+//
+// Consumers split the tile by ROWS: warpgroup h owns tile rows 64h .. 64h + 63 (pixel rows 8h .. 8h + 7) and all BN
+// columns, warp w rows 16w .. 16w + 15.  Each warp loads its A rows once per tap and each warpgroup issues one
+// m64nBNk16 per k16 step.  BN is a template parameter, so every wgmma has a fixed shape and none sits under a
+// data-dependent branch: the last n-tile issues all BN columns (the packed weight rows beyond N are zero) and the
+// zero-padded last 64-channel chunk of a source issues all four k16 steps (its pad channels are TMA zero fill, or
+// zeros written by the resample warps).  The mainloop keeps one tap's wgmma group in flight while the next tap's A
+// fragments load.
 constexpr int kHaloW = 10, kHaloH = 18;
 constexpr int kHaloBytes = kHaloW * kHaloH * 128;          // 23040
 constexpr int kHaloSlot = 24 * 1024;                        // 1024-B aligned slot
 constexpr int kHaloSlots = 3;
+constexpr int kMaxSmem = 227 * 1024;
+constexpr int kHaloXposeWarp = 16 * 32 * 4;                 // per consumer warp: 16 x 32 fp32 accumulator transpose
+constexpr int kHaloBarBytes = 512;
+// shared memory left for the weight ring next to the halo slots, transposes and barriers
+constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kHaloBarBytes - kEpiWarps * kHaloXposeWarp - kHaloSlots * kHaloSlot;
+// taps per weight stage: amortise the per-stage barrier round trip over several taps while two stages still fit
+__host__ __device__ constexpr int halo_kc(int bn) {
+  return 2 * 9 * bn * kBlockK * 2 <= kHaloBBytes ? 9 : (2 * 3 * bn * kBlockK * 2 <= kHaloBBytes ? 3 : 1);
+}
+// weight ring depth: as many stages of halo_kc taps as fit (at least two by the choice of halo_kc), at most six
+__host__ __device__ constexpr int halo_stages(int bn) {
+  return kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) < 6 ? kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) : 6;
+}
 
 
 // ---- fused bilinear resample (align_corners=True) of a halo-kernel source -------------------------------------------
@@ -845,28 +873,105 @@ __device__ __forceinline__ void halo_fill_bilinear(uint32_t slot, const GemmDesc
   }
 }
 
+// A fragments of one tap for this warp's 16 rows: lane l addresses its row (ra = the row's 128-byte halo pixel),
+// 16-byte chunk 2k + (l >> 4) of k16 step k (SWIZZLE_128B: chunk j of the row at address a sits at j ^ ((a >> 7) & 7)).
+__device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&fa)[4][4]) {
+  const uint32_t sw = (ra >> 7) & 7;
+#pragma unroll
+  for (int k = 0; k < kBlockK / 16; ++k) ldmatrix_x4(ra + (((2 * k + (lane >> 4)) ^ sw) << 4), fa[k]);
+}
+
+// Accumulator fragment -> one row half per thread.  A warp holds rows 16w .. 16w + 15 of the tile in one m64nBN
+// fragment: element 4j + e at (row lane/4, column 8j + 2(lane%4) + e), 4j + 2 + e at row lane/4 + 8.  acc_stage16<K>
+// writes columns 32K .. 32K + 31 into the warp's 16 x 32 fp32 block; lane l then reads row l & 15, columns
+// 16 (l >> 4) .. + 15.  Word (r, c) sits at r * 32 + (c ^ s(r)), s mapping row bits 0, 1, 2, 3 to bits 0, 3, 2 + 4, 1:
+// the fragment writes (8 rows x 4 column pairs) and the row reads (16 rows x 2 halves) each touch 32 distinct banks.
+__device__ __forceinline__ int xpose16_swz(int r) { return (r & 1) | ((r & 8) >> 2) | (r & 4) | ((r & 2) << 2) | ((r & 4) << 2); }
+template <int K, int S>
+__device__ __forceinline__ void acc_stage16(const float (&a)[S], float* buf, int lane) {
+  const int r0 = lane >> 2, cl = 2 * (lane & 3);
+#pragma unroll
+  for (int jj = 0; jj < 4; ++jj) {
+    const int j = 4 * K + jj;
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = 8 * jj + cl + e;
+      buf[r0 * 32 + (c ^ xpose16_swz(r0))] = a[4 * j + e];
+      buf[(r0 + 8) * 32 + (c ^ xpose16_swz(r0 + 8))] = a[4 * j + 2 + e];
+    }
+  }
+}
+// runtime chunk index (uniform over the warp, k < S / 16); register indices stay compile-time
+template <int S>
+__device__ __forceinline__ void acc_stage16_k(int k, const float (&a)[S], float* buf, int lane) {
+  constexpr int kLast = S / 16 - 1;
+  if (k == 0) acc_stage16<0>(a, buf, lane);
+  else if (k == 1) acc_stage16<(1 < kLast ? 1 : kLast)>(a, buf, lane);
+  else if (k == 2) acc_stage16<(2 < kLast ? 2 : kLast)>(a, buf, lane);
+  else if (k == 3) acc_stage16<(3 < kLast ? 3 : kLast)>(a, buf, lane);
+  else if (k == 4) acc_stage16<(4 < kLast ? 4 : kLast)>(a, buf, lane);
+  else acc_stage16<kLast>(a, buf, lane);
+}
+
+// The 32-column chunks of the tile that hold columns < N; each thread takes 16 columns of its row per chunk.
+template <int TAILN, int S>
+__device__ __forceinline__ void halo_epilogue_row(const GemmDesc& d, const float (&acc)[S], float* buf, int lane,
+                                                  const TileCoord& c, long long orow, bool row_ok, float (&y2)[kMaxTail]) {
+  const int r = lane & 15;
+  const float* rowp = buf + r * 32;
+  const int sw = xpose16_swz(r) ^ (lane & 16);     // column 16 (lane >> 4) + j of row r is word j ^ sw of rowp
+  for (int k = 0; 32 * k < 2 * S && c.n0 + 32 * k < d.N; ++k) {
+    acc_stage16_k(k, acc, buf, lane);
+    __syncwarp();
+    epilogue_cols<16, TAILN>(d, rowp, sw, 32 * k + (lane & 16), c, c.n0, orow, row_ok, y2);
+    __syncwarp();
+  }
+}
+
+template <int S>
+__device__ __forceinline__ void halo_epilogue_tile(const GemmDesc& d, const TileCoord& c, const float (&acc)[S], int warp,
+                                                   int lane, float* buf) {
+  const int r = 16 * warp + (lane & 15);           // tile row (bw = 8): pixel (r / 8, r % 8) of the 16 x 8 tile
+  const int y = c.y0 + (r >> 3), x = c.x0 + (r & 7);
+  const bool row_ok = (y < d.H) && (x < d.W) && (c.img < d.NB);   // img >= NB: phantom tile of a multicast cluster
+  const long long orow = (static_cast<long long>(c.img) * d.H + y) * d.W + x;
+  float y2[kMaxTail];
+#pragma unroll
+  for (int i = 0; i < kMaxTail; ++i) y2[i] = 0.f;
+  if (d.w2 == nullptr) halo_epilogue_row<0>(d, acc, buf, lane, c, orow, row_ok, y2);
+  else if (d.n2 <= 1) halo_epilogue_row<1>(d, acc, buf, lane, c, orow, row_ok, y2);
+  else if (d.n2 <= 4) halo_epilogue_row<4>(d, acc, buf, lane, c, orow, row_ok, y2);
+  else halo_epilogue_row<kMaxTail>(d, acc, buf, lane, c, orow, row_ok, y2);
+  if (d.w2 != nullptr) {
+    // lanes l and l ^ 16 hold the fused trailing layer's partial sums over alternate 16-column halves of one row
+#pragma unroll
+    for (int i = 0; i < kMaxTail; ++i)
+      if (i < d.n2) y2[i] += __shfl_xor_sync(0xffffffffu, y2[i], 16);
+    if (row_ok && lane < 16) tail_store(d, orow, y2);
+  }
+}
+
 // CL > 1: clusters of CL (2 or 4) CTAs take CL m-tiles (pixel tiles) of the SAME n-tile; each CTA fetches 1/CL of the rows
 // of every weight tile and multicasts it into all of them.  The weights are ~90 % of this kernel's L2 -> SM traffic (one
-// 23 KB halo against nine 16-32 KB tap tiles per 64-channel chunk).
-template <int CL, int S>
+// 23 KB halo against nine 4-24 KB tap tiles per 64-channel chunk).
+template <int CL, int BN>
 __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __grid_constant__ GemmKernelParams P) {
   constexpr bool MC = CL > 1;
   constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1);
+  constexpr int kc = halo_kc(BN);                           // taps per B stage
+  constexpr int b_tile_bytes = BN * kBlockK * 2;
+  constexpr int b_stage_bytes = kc * b_tile_bytes;
+  constexpr int stages = halo_stages(BN);                   // B ring
   extern __shared__ uint8_t smem_raw[];
   const GemmDesc& d = P.d;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int stages = P.stages;                              // B ring
-  const int kc = P.kc;                                      // taps per B stage
-  const int b_tile_bytes = d.block_n * kBlockK * 2;
-  const int b_stage_bytes = kc * b_tile_bytes;
   uint8_t* smem_b = smem + kHaloSlots * kHaloSlot;
-  uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][4 KB] accumulator transposes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiStageBytes);
+  uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][2 KB] accumulator transposes
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kHaloXposeWarp);
   uint64_t* a_full = bars;                                  // [kHaloSlots]
   uint64_t* a_empty = a_full + kHaloSlots;
   uint64_t* b_full = a_empty + kHaloSlots;                  // [stages]
   uint64_t* b_empty = b_full + stages;
-  float* tail_smem = reinterpret_cast<float*>(bars + 64);   // [128][kMaxTail]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -909,7 +1014,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
               if (elect_one()) {
                 mbar_expect_tx(&b_full[bs], b_stage_bytes);
                 if (MC) {
-                  const int part_rows = d.block_n / CL;
+                  constexpr int part_rows = BN / CL;
                   for (int j = 0; j < kc; ++j)
                     tma_load_2d_mc(smem_b + bs * b_stage_bytes + j * b_tile_bytes + it.rank * part_rows * 128, &P.tmBh,
                                    &b_full[bs], (kbase + (tap0 + j) * nch + ch) * kBlockK, c.n0 + it.rank * part_rows,
@@ -950,46 +1055,51 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma over the nine shifted views of each halo tile + epilogue =====
-    const int q = warp & 3, half = warp >> 2;
-    float* buf = reinterpret_cast<float*>(xpose + warp * kStageTile);
-    const uint32_t b_off = static_cast<uint32_t>(half * (d.block_n >> 1) * 128);
-    float a0[S], a1[S];
+    float* buf = reinterpret_cast<float*>(xpose + warp * kHaloXposeWarp);
+    const int arow = 16 * warp + (lane & 15);               // tile row this lane addresses for ldmatrix
+    const uint32_t a_off = static_cast<uint32_t>(((arow >> 3) * kHaloW + (arow & 7)) * 128);
+    float acc[BN / 2];
+    uint32_t fa[2][4][4];                                   // A fragments of two taps: one loads while the other is read
     int as = 0; uint32_t aph = 0;
     int bs = 0; uint32_t bph = 0;
+    int rbs = 0;                                            // oldest B stage not yet released
     for (int ti = it.first; ti < it.count; ti += it.step) {
-      const int t = it.tile(ti);
-      const TileCoord c = decode_tile(d, t);
-      const int nw = half_n(d, t, half);
+      const TileCoord c = decode_tile(d, it.tile(ti));
       uint32_t accum = 0;
       for (int s = 0; s < d.num_src; ++s) {
-        const int nk_last = last_chunk_k16(d, s);
         for (int ch = 0; ch < d.chunks[s]; ++ch) {
-          const int nk = ch == d.chunks[s] - 1 ? nk_last : kBlockK / 16;
           mbar_wait(&a_full[as], aph);
-          const uint32_t halo = smem_u32(smem + as * kHaloSlot);
-          for (int tap0 = 0; tap0 < 9; tap0 += kc) {
-            mbar_wait(&b_full[bs], bph);
-            if (nw > 0) {
-              const uint32_t sb = smem_u32(smem_b + bs * b_stage_bytes) + b_off;
-              for (int j = 0; j < kc; ++j) {
-                const int tap = tap0 + j;
-                const int dy = tap / 3, dx = tap - dy * 3;
-                uint32_t fa[2][4][4];
-                load_a_frags([halo, dy, dx](int row) {
-                  return halo + static_cast<uint32_t>((((row >> 3) + dy) * kHaloW + (row & 7) + dx) * 128);
-                }, q, lane, nk, fa);
-                mma_block(a0, a1, fa, wgmma_desc_k128(sb + j * b_tile_bytes), nw, nk, accum);
-                accum = 1;
-              }
+          const uint32_t a_base = smem_u32(smem + as * kHaloSlot) + a_off;
+          uint32_t sb = 0;
+#pragma unroll
+          for (int tap = 0; tap < 9; ++tap) {
+            if (tap % kc == 0) {
+              mbar_wait(&b_full[bs], bph);
+              sb = smem_u32(smem_b + bs * b_stage_bytes);
+              if (++bs == stages) { bs = 0; bph ^= 1; }
             }
-            release_stage<CL>(&b_empty[bs], lane);
-            if (++bs == stages) { bs = 0; bph ^= 1; }
+            // fa[tap & 1] was last read by the group of tap - 2, retired by the wait below at tap - 1
+            halo_a_frags(a_base + static_cast<uint32_t>(((tap / 3) * kHaloW + tap % 3) * 128), lane, fa[tap & 1]);
+            const uint64_t bdesc = wgmma_desc_k128(sb + (tap % kc) * b_tile_bytes);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k) Wgmma<BN>::rs(acc, fa[tap & 1][k], bdesc + 2 * k, accum | k);
+            wgmma_commit();
+            accum = 1;
+            wgmma_wait<1>();                                 // the group of tap - 1 is done
+            if (tap > 0 && tap % kc == 0) {                  // ... and it was the last reader of its B stage
+              release_stage<CL>(&b_empty[rbs], lane);
+              if (++rbs == stages) rbs = 0;
+            }
           }
-          release_stage<1>(&a_empty[as], lane);             // halo slot reusable once its 9 taps are done
+          wgmma_wait<0>();                                   // tap 8 is done: its B stage and the halo slot are free
+          release_stage<CL>(&b_empty[rbs], lane);
+          if (++rbs == stages) rbs = 0;
+          release_stage<1>(&a_empty[as], lane);
           if (++as == kHaloSlots) { as = 0; aph ^= 1; }
         }
       }
-      epilogue_tile(d, c, a0, a1, warp, lane, buf, tail_smem, nullptr);
+      halo_epilogue_tile(d, c, acc, warp, lane, buf);
       __syncwarp();
     }
   }
@@ -1003,19 +1113,33 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
 // ------------------------------------------------------------------------------------------------------------
 static int g_sm_counts[kMaxDevices] = {0};
 
+using KernelFn = void (*)(GemmKernelParams);
+// pf_conv3_halo_kernel<CL, bn>, nullptr for a width without an instantiation
+template <int CL>
+static KernelFn halo_kernel_cl(int bn) {
+  switch (bn) {
+    case 32: return pf_conv3_halo_kernel<CL, 32>;
+    case 64: return pf_conv3_halo_kernel<CL, 64>;
+    case 128: return pf_conv3_halo_kernel<CL, 128>;
+    case 192: return pf_conv3_halo_kernel<CL, 192>;
+    default: return nullptr;
+  }
+}
+static KernelFn halo_kernel(int cl, int bn) {
+  return cl == 4 ? halo_kernel_cl<4>(bn) : (cl == 2 ? halo_kernel_cl<2>(bn) : halo_kernel_cl<1>(bn));
+}
+
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
                 const CUtensorMap* tmOut, cudaStream_t stream) {
   static bool attr_done[kMaxDevices] = {false};
-  const int kMaxSmem = 227 * 1024;
   const int dev = current_device();
   if (!attr_done[dev]) {
     cudaError_t e = cudaSuccess;
-    for (void* k : {reinterpret_cast<void*>(pf_gemm_kernel<false, 32>), reinterpret_cast<void*>(pf_gemm_kernel<false, 64>),
-                    reinterpret_cast<void*>(pf_gemm_kernel<true, 32>), reinterpret_cast<void*>(pf_gemm_kernel<true, 64>),
-                    reinterpret_cast<void*>(pf_conv3_halo_kernel<1, 32>), reinterpret_cast<void*>(pf_conv3_halo_kernel<1, 64>),
-                    reinterpret_cast<void*>(pf_conv3_halo_kernel<2, 32>), reinterpret_cast<void*>(pf_conv3_halo_kernel<2, 64>),
-                    reinterpret_cast<void*>(pf_conv3_halo_kernel<4, 32>), reinterpret_cast<void*>(pf_conv3_halo_kernel<4, 64>)})
+    for (KernelFn k : {pf_gemm_kernel<false, 32>, pf_gemm_kernel<false, 64>, pf_gemm_kernel<true, 32>, pf_gemm_kernel<true, 64>})
       if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    for (int cl : {1, 2, 4})
+      for (int bn : {32, 64, 128, 192})
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm kernels): %s", cudaGetErrorString(e));
     cudaDeviceGetAttribute(&g_sm_counts[dev], cudaDevAttrMultiProcessorCount, dev);
     attr_done[dev] = true;
@@ -1041,7 +1165,6 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   P.tmOut = tmOut ? *tmOut : tmB;
   P.d = d;
   if (d.tma_out && !tmOut) return set_error("gemm: tma_out without an output tensor map");
-  P.kc = 1;
   int stage_bytes = kATileBytes + d.block_n * kBlockK * 2;
   int budget = kMaxSmem - 1024 /*align*/ - kEpiSmemBytes /*barriers, fused-tail scratch, transpose / staging blocks*/;
   int stages = budget / stage_bytes;
@@ -1056,22 +1179,13 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   int grid = P.total_tiles < g_sm_count ? P.total_tiles : g_sm_count;
   size_t smem = 1024 + static_cast<size_t>(stages) * stage_bytes + kEpiSmemBytes;
   if (d.halo) {
-    int b_bytes = d.block_n * kBlockK * 2;
-    int hb = kMaxSmem - 1024 - kTailBytes - kEpiStageBytes - kHaloSlots * kHaloSlot;
-    // taps per weight stage: amortise the per-stage barrier round trip over several taps of MMA work
-    int kc = 1;
-    if (9 * b_bytes * 2 <= hb) kc = 9;
-    else if (3 * b_bytes * 2 <= hb && d.block_n < 256) kc = 3;
-    static const int kc_force = getenv("PF_B200_HALO_KC") ? atoi(getenv("PF_B200_HALO_KC")) : 0;   // tuning hook
-    if ((kc_force == 1 || kc_force == 3 || kc_force == 9) && kc_force * b_bytes * 2 <= hb) kc = kc_force;
-    P.kc = kc;
-    b_bytes *= kc;
-    int hstages = hb / b_bytes;
-    if (hstages > 6) hstages = 6;
-    if (hstages < 2) return set_error("conv3 halo: not enough shared memory");
+    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n);
+    if (hk == nullptr) return set_error("conv3 halo: block_n %d (32, 64, 128 or 192)", d.block_n);
+    const int b_bytes = halo_kc(d.block_n) * d.block_n * kBlockK * 2;     // one weight stage
+    const int hstages = halo_stages(d.block_n);
     P.stages = hstages;
     size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * kHaloSlot + static_cast<size_t>(hstages) * b_bytes +
-                   kEpiStageBytes + kTailBytes;
+                   kEpiWarps * kHaloXposeWarp + kHaloBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
       // weight-multicast clusters of cl CTAs over (m-tile group, n-tile) work items.  Every CTA is persistent, so the grid
@@ -1091,19 +1205,16 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       if (max_clusters[dev][cl] == 0) {
         cfg.gridDim = dim3(cl * (g_sm_count / cl));
         int n = 0;
-        cudaError_t qe = cl == 2 ? cudaOccupancyMaxActiveClusters(&n, pf_conv3_halo_kernel<2, 64>, &cfg)
-                                 : cudaOccupancyMaxActiveClusters(&n, pf_conv3_halo_kernel<4, 64>, &cfg);
+        cudaError_t qe = cudaOccupancyMaxActiveClusters(&n, hk, &cfg);
         if (qe != cudaSuccess || n < 1) { cudaGetLastError(); n = g_sm_count / cl; }
         max_clusters[dev][cl] = n < g_sm_count / cl ? n : g_sm_count / cl;
       }
       const int clusters = groups < max_clusters[dev][cl] ? groups : max_clusters[dev][cl];
       cfg.gridDim = dim3(cl * clusters);
       cfg.numAttrs = pdl_enabled() ? 2 : 1;
-      if (cl == 2) le = wide_acc ? cudaLaunchKernelEx(&cfg, pf_conv3_halo_kernel<2, 64>, P) : cudaLaunchKernelEx(&cfg, pf_conv3_halo_kernel<2, 32>, P);
-      else le = wide_acc ? cudaLaunchKernelEx(&cfg, pf_conv3_halo_kernel<4, 64>, P) : cudaLaunchKernelEx(&cfg, pf_conv3_halo_kernel<4, 32>, P);
+      le = cudaLaunchKernelEx(&cfg, hk, P);
     } else {
-      le = wide_acc ? launch_pdl(pf_conv3_halo_kernel<1, 64>, dim3(grid), dim3(kHaloThreads), hsmem, stream, P)
-                    : launch_pdl(pf_conv3_halo_kernel<1, 32>, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
+      le = launch_pdl(hk, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
     }
     if (le != cudaSuccess) return set_error("pf_conv3_halo_kernel launch: %s", cudaGetErrorString(le));
   } else if (tmBh != nullptr) {
