@@ -322,45 +322,22 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
     if (u->a_c[s] % 8 || u->a_ld[s] % 8) return set_error("pf_gemm: source %d channels/ld must be multiples of 8", s);
   }
   if (u->Ktot != ksteps * 64) return set_error("pf_gemm: Ktot %d != %d expected from sources", u->Ktot, ksteps * 64);
-  // N tiling
-  int bn = u->block_n;
-  if (bn == 0 && u->ps > 1) {
-    // pixel shuffle: an N tile must not straddle two (ky,kx) taps
-    int cpad = (u->ps_cout + 31) / 32 * 32;
-    for (int c = 256; c >= 32; c -= 32)
-      if (cpad % c == 0) { bn = c; break; }
-  }
-  if (bn == 0) {
-    int n32 = (u->N + 31) / 32 * 32;
-    if (n32 <= 256) bn = n32;
-    else {
-      // largest multiple of 32 in [128,256] minimising padded columns
-      int bestpad = 1 << 30;
-      for (int c = 256; c >= 128; c -= 32) {
-        int pad = (u->N + c - 1) / c * c - u->N;
-        if (pad < bestpad) { bestpad = pad; bn = c; }
-      }
+  // N tiling.  The packed weight panel has n_pad rows (ops.n_pad_for): N rounded up to 32 up to 256, above that to a
+  // multiple of the width in [128, 256] that pads least.  Every n-tile width chosen below divides n_pad, so the last
+  // n-tile reads zero-packed rows only.
+  int n_pad = (u->N + 31) / 32 * 32;
+  if (n_pad > 256) {
+    int bestpad = 1 << 30, pw = 256;
+    for (int c = 256; c >= 128; c -= 32) {
+      int pad = (u->N + c - 1) / c * c - u->N;
+      if (pad < bestpad) { bestpad = pad; pw = c; }
     }
+    n_pad = (u->N + pw - 1) / pw * pw;
   }
   // 3x3 convs go through the halo-tile kernel (one A fetch per 64-channel chunk instead of nine) unless the caller
   // pins a tile shape or PF_B200_NO_HALO is set.
   static const bool no_halo = getenv("PF_B200_NO_HALO") != nullptr;
   const bool halo = u->a_mode == 1 && u->taps == 9 && u->bh == 0 && u->bw == 0 && !no_halo;
-  if (halo && u->block_n == 0) {
-    // The halo kernel is compiled for block_n 32, 64, 128 and 192 (a warpgroup's 64 x block_n fp32 accumulator in
-    // registers): the widest that divides the packed panel's rows, so the last n-tile reads zero-packed rows only.  A
-    // fused trailing layer wider than that is refused below (it needs the whole row in one n-tile).
-    const int n_pad = (u->N + bn - 1) / bn * bn;
-    bn = n_pad % 192 == 0 ? 192 : (n_pad % 128 == 0 ? 128 : (n_pad % 64 == 0 ? 64 : 32));
-  } else if (!halo && u->block_n == 0 && bn > 128 && bn % 64 == 0 && !u->w2) {
-    // pf_gemm_kernel holds the 128 x block_n fp32 accumulator tile in the registers of two consumer warpgroups; half
-    // tiles of up to 64 columns leave the epilogue room without spilling.  A 192- or 256-column choice (the packed
-    // weights stay padded for it) therefore runs as two n-tiles of half the width, unless a fused trailing layer needs
-    // the whole row in one tile.
-    bn /= 2;
-  }
-  d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
-  u->block_n = bn; u->n_tiles = d.n_tiles;
   d.M = u->M; d.NB = u->NB; d.H = u->H; d.W = u->W;
   CUtensorMap tmA[3], tmB;
   d.halo = halo ? 1 : 0;
@@ -409,8 +386,35 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
       if (tmap_2d_bf16(&tmA[s], u->a_ptr[s], u->a_c[s], u->M, u->a_ld[s], 64, 128)) return 1;
   }
   u->bh = d.bh; u->bw = d.bw; u->tiles_y = d.tiles_y; u->tiles_x = d.tiles_x; u->m_tiles = d.m_tiles;
-  int n_pad = d.n_tiles * bn;
-  if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, n_pad, u->Ktot, 64, bn)) return 1;
+  // Both kernels hold a warpgroup's 64 x block_n fp32 accumulator tile in registers and are compiled per width
+  // (pf_gemm_kernel: kGemmWidths; halo kernel: 32, 64, 128 and 192).
+  int bn = u->block_n;
+  if (bn == 0) {
+    if (halo) {
+      // the widest halo width that divides the panel; a fused trailing layer wider than that is refused below
+      bn = n_pad % 192 == 0 ? 192 : (n_pad % 128 == 0 ? 128 : (n_pad % 64 == 0 ? 64 : 32));
+    } else if (u->ps > 1 || u->w2) {
+      // pixel shuffle: an n-tile must not straddle two (ky,kx) taps (the widest width dividing the padded Cout); a
+      // fused trailing layer needs the whole row in one n-tile
+      const int span = u->ps > 1 ? (u->ps_cout + 31) / 32 * 32 : n_pad;
+      for (int w : kGemmWidths)
+        if (span % w == 0) bn = w;
+      if (u->w2 && bn != n_pad) return set_error("pf_gemm: fused trailing layer needs the whole row in one N tile (N %d)", u->N);
+    } else if (n_pad % 128 == 0) {
+      // 128 or 256 columns: a 256-column tile reads less shared memory per MMA, but halves the tile count.  Take 256
+      // unless it needs more waves of tiles over the SMs for the same columns (N = 1024 at 73 m-tiles: 584 tiles of 128
+      // are 4.4 waves on 132 SMs, 292 tiles of 256 are 2.2 waves, so 128 finishes first).
+      const long long t128 = static_cast<long long>(d.m_tiles) * (n_pad / 128), sms = sm_count();
+      const long long waves128 = (t128 + sms - 1) / sms, waves256 = (t128 / 2 + sms - 1) / sms;
+      bn = n_pad % 256 == 0 && 2 * waves256 <= waves128 ? 256 : 128;
+    } else {
+      for (int w : kGemmWidths)
+        if (n_pad % w == 0) bn = w;
+    }
+  }
+  d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
+  u->block_n = bn; u->n_tiles = d.n_tiles;
+  if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) return 1;
   d.bias = u->bias; d.act = u->act;
   d.res1 = static_cast<const __nv_bfloat16*>(u->res1);
   d.res2 = static_cast<const __nv_bfloat16*>(u->res2);
@@ -456,7 +460,7 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   d.halo_cl = halo ? cl : 1;
   const bool mc = cl > 1;
   CUtensorMap tmBh;
-  if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, n_pad, u->Ktot, 64, bn / cl)) return 1;
+  if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)) return 1;
   // Epilogue through shared memory + TMA (pf_gemm_kernel only): plain bf16 outputs in 64-column groups, fp32 outputs
   // and the fp32 residual stream (x += gamma * v) in 32-column chunks.  PF_OPT_TMA_EPILOGUE = 0 keeps the direct stores.
   const bool no_tma_epi = option(PF_OPT_TMA_EPILOGUE) == 0;
@@ -464,17 +468,17 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   d.tma_out = 0;
   if (!no_tma_epi && !halo && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2) {
     const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;     // columns >= N are clipped by the copy
-    // each consumer warpgroup stores whole 64-column groups (bf16) / 32-column chunks (fp32) of its half of the tile
-    if (!d.out_f32 && bn % 128 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
+    // each consumer warp stores its 16 rows in whole 64-column groups (bf16) / 32-column chunks (fp32)
+    if (!d.out_f32 && bn % 64 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
       if (u->a_mode == 0) {
-        if (tmap_2d_bf16(&tmOut, u->out, ocols, u->M, u->out_ld, 64, 32)) return 1;
+        if (tmap_2d_bf16(&tmOut, u->out, ocols, u->M, u->out_ld, 64, 16)) return 1;
       } else {
-        const uint32_t bwx = d.bw < 32 ? d.bw : 32;
-        if (tmap_4d_nhwc_bf16(&tmOut, u->out, ocols, u->W, u->H, u->NB, u->out_ld, 64, bwx, 32 / bwx)) return 1;
+        const uint32_t bwx = d.bw < 16 ? d.bw : 16;
+        if (tmap_4d_nhwc_bf16(&tmOut, u->out, ocols, u->W, u->H, u->NB, u->out_ld, 64, bwx, 16 / bwx)) return 1;
       }
       d.tma_out = 1;
-    } else if (d.out_f32 && bn % 64 == 0 && u->a_mode == 0 && u->out_ld % 4 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
-      if (tmap_2d_f32(&tmOut, u->out, ocols, u->M, u->out_ld, 32, 32)) return 1;
+    } else if (d.out_f32 && u->a_mode == 0 && u->out_ld % 4 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
+      if (tmap_2d_f32(&tmOut, u->out, ocols, u->M, u->out_ld, 32, 16)) return 1;
       d.tma_out = 2;
     }
   }

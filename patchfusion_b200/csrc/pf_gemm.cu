@@ -15,17 +15,22 @@
 // rows, so there is no im2col buffer and no halo code.  Weights are pre-packed K-major [N, Ktot] with every
 // (source, tap) segment padded to a multiple of 64 channels, matching the producer's enumeration order.
 //
-// Warp roles (pf_gemm_kernel; the halo kernel below splits its tile by rows instead): warps 0-7 = two consumer
-// warpgroups.  Warpgroup h computes columns [h * block_n / 2,
-// (h + 1) * block_n / 2) of the 128-row tile with wgmma (A fragments loaded by ldmatrix from the swizzled TMA tile, B
-// read by the tensor core from shared memory); warp w of a warpgroup owns tile rows 32 (w & 3) .. 32 (w & 3) + 31,
-// fed to the instruction as two 16-row halves, so after the mainloop every accumulator row lives in one warp.  The
-// same warps then run the epilogue: a 32 x 32 fp32 block at a time goes through a per-warp swizzled shared-memory
-// transpose so that one thread holds one accumulator row (bias / activation / residuals / fused tail per row), then a
-// swizzled staging tile + bulk tensor store (bf16), a bulk reduce-add (the fp32 residual stream), or direct stores for
-// the fused-tail / residual / pixel-shuffle / V^T variants.  The last warp is the TMA producer; the halo kernel has
-// two more warps before it, the operand producers of its optional fused bilinear resample (idle otherwise).  While the consumers drain a tile, the
-// producer already fills the operand ring for the next one.
+// Warp roles (pf_gemm_kernel): warps 0-7 = two consumer warpgroups.  Warpgroup h computes tile rows 64h .. 64h + 63
+// against all BN columns of the n-tile, one wgmma.m64nBNk16 per k16 step with both operands read by the tensor core
+// from the swizzled TMA tiles in shared memory (every A tile is 128 rows x 128 B in the canonical K-major layout, so
+// the warpgroup's A operand is a descriptor at its 8 KB row offset).  Warp w owns tile rows 16w .. 16w + 15, so after
+// the mainloop every accumulator row lives in one warp.  The same warps then run the epilogue: a 16 x 32 fp32 block at
+// a time goes through a per-warp swizzled shared-memory transpose so that a thread holds 16 columns of one accumulator
+// row (bias / activation / residuals / fused tail per row), then a swizzled staging tile + bulk tensor store (bf16), a
+// bulk reduce-add (the fp32 residual stream), or direct stores for the fused-tail / residual / pixel-shuffle / V^T
+// variants.  The last warp is the TMA producer; the halo kernel has two more warps before it, the operand producers of
+// its optional fused bilinear resample (idle otherwise).  While the consumers drain a tile, the producer already fills
+// the operand ring for the next one.
+//
+// BN is a template parameter of both kernels, so every wgmma has a fixed shape and none sits under a data-dependent
+// branch: the last n-tile issues all BN columns (the packed weight rows beyond N are zero, the epilogue drops those
+// columns) and the zero-padded last 64-channel chunk of a source issues all four k16 steps (its pad channels are TMA
+// zero fill against zero-packed weights).
 #include "pf_common.cuh"
 #include "pf_kernels.h"
 
@@ -36,21 +41,34 @@ constexpr int kBlockK = 64;
 constexpr int kATileBytes = kBlockM * kBlockK * 2;  // 16 KiB
 constexpr int kEpiWarps = 8;                       // consumer warps: two warpgroups
 // pf_gemm_kernel: consumers + one TMA producer warp; pf_conv3_halo_kernel: + two resample producer warps before it.
-// A consumer thread holds up to 2 x 64 (pf_gemm_kernel) or 96 (halo kernel) fp32 accumulators plus 32 A-fragment
-// registers: no idle warps, so that the per-thread register budget (65536 / threads, capped at 168) stays large.
+// A consumer thread holds BN / 2 fp32 accumulators (plus 32 A-fragment registers in the halo kernel): no idle warps,
+// so that the per-thread register budget (65536 / threads, capped at 168) stays large.
 constexpr int kGemmThreads = (kEpiWarps + 1) * 32;
 constexpr int kHaloThreads = (kEpiWarps + 3) * 32;
 constexpr int kRsWarp0 = kEpiWarps;                         // halo kernel: warps 8, 9 = resample producers
+constexpr int kMaxSmem = 227 * 1024;
+// per consumer warp: the 16 x 32 fp32 accumulator transpose; in pf_gemm_kernel also the staging tile (16 rows x 128 B,
+// SWIZZLE_128B) of the TMA-store epilogue
+constexpr int kXposeWarp = 16 * 32 * 4;
+constexpr int kBarBytes = 512;
+
+// pf_gemm_kernel operand ring: one stage = the 128-row A tile + BN weight rows of one 64-wide K block; as many stages
+// as fit next to the transposes and barriers, at most eight
+__host__ __device__ constexpr int gemm_stage_bytes(int bn) { return kATileBytes + bn * kBlockK * 2; }
+__host__ __device__ constexpr int gemm_stages(int bn) {
+  return (kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kXposeWarp) / gemm_stage_bytes(bn) < 8
+             ? (kMaxSmem - 1024 - kBarBytes - kEpiWarps * kXposeWarp) / gemm_stage_bytes(bn)
+             : 8;
+}
 
 struct GemmKernelParams {
   CUtensorMap tmA[3];
   CUtensorMap tmB;
   CUtensorMap tmBh;     // multicast variant: box of block_n / cl weight rows (each CTA of the cluster fetches one part)
-  CUtensorMap tmOut;    // d.tma_out: output tensor (bf16 {64 cols, 32 rows} boxes, or fp32 {32 cols, 32 rows})
+  CUtensorMap tmOut;    // d.tma_out: output tensor (bf16 {64 cols, 16 rows} boxes, or fp32 {32 cols, 16 rows})
   GemmDesc d;
-  int stages;
   int total_tiles;
-  int k_steps;  // per tile
+  int k_steps;  // 64-wide K blocks per tile
 };
 
 
@@ -77,32 +95,14 @@ __device__ __forceinline__ TileCoord decode_tile(const GemmDesc& d, int t) {
   return c;
 }
 
-
-// Columns the MMA of tile t must produce: block_n, or for the last n-tile the remaining columns rounded up to 16.
-__device__ __forceinline__ int tile_n_eff(const GemmDesc& d, int t) {
-  const int n0 = (t % d.n_tiles) * d.block_n;
-  const int rem = ((d.N - n0 + 15) >> 4) << 4;
-  return rem < d.block_n ? rem : d.block_n;
-}
-// K = 16 steps that carry data in the last 64-channel chunk of source s (the rest of the chunk is TMA zero fill).
-__device__ __forceinline__ int last_chunk_k16(const GemmDesc& d, int s) {
-  return (d.k_true[s] - (d.chunks[s] - 1) * kBlockK + 15) >> 4;
-}
-
-// One 32-column chunk of one accumulator row: bias -> activation -> residuals -> store.  FULL == all 32 columns exist
+// One W-column chunk of one accumulator row: bias -> activation -> residuals -> store.  FULL == all W columns exist
 // (vector loads/stores, no predication); the tail variant predicates every column but keeps all indices static so
 // f[] stays in registers.
 constexpr int kMaxTail = 16;   // widest fused trailing 1x1 layer
-constexpr int kTailBytes = 512 + 128 * kMaxTail * 4;   // barriers + [128][kMaxTail] fp32 scratch
-// one 4 KB block per consumer warp: the 32 x 32 fp32 accumulator transpose, and in pf_gemm_kernel also the staging tile
-// (32 rows x 128 B, SWIZZLE_128B) of the TMA-store epilogue
-constexpr int kStageTile = 32 * 128;
-constexpr int kEpiStageBytes = kEpiWarps * kStageTile;  // 32 KB
-constexpr int kEpiSmemBytes = kTailBytes + kEpiStageBytes;
 
-// W = chunk width in accumulator columns (32, or 16 for the last chunk of a half tile of 16 mod 32 columns);
-// TAILN = compile-time bound on the fused trailing layer's outputs (0 = no trailing layer): keeps the executed code
-// path short - the fully unrolled 16-output variant alone is ~3k instructions and thrashed the instruction cache.
+// W = chunk width in accumulator columns; TAILN = compile-time bound on the fused trailing layer's outputs (0 = no
+// trailing layer): keeps the executed code path short - the fully unrolled 16-output variant alone is ~3k
+// instructions and thrashed the instruction cache.
 template <bool FULL, int W, int TAILN>
 __device__ __forceinline__ void epilogue_chunk(const GemmDesc& d, float (&f)[W], long long orow, int ncol, int lcol,
                                                int nvalid, float (&y2)[kMaxTail], uint32_t (&xv)[TAILN == 0 ? W / 8 : 1][8]) {
@@ -275,15 +275,14 @@ __device__ __forceinline__ void epilogue_chunk(const GemmDesc& d, float (&f)[W],
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Accumulator fragments -> one row per thread.  A consumer warp holds rows 32q .. 32q + 31 of the tile (q = warp & 3)
-// in two wgmma fragments: acc0 = rows +0..15, acc1 = rows +16..31, element 4j + e of a fragment at (row lane/4,
-// column 8j + 2(lane%4) + e) and 4j + 2 + e at row lane/4 + 8.  acc_stage<K> writes accumulator columns 32K .. 32K + 31
-// into the warp's 32 x 32 fp32 block; acc_read gives thread `lane` row `lane`.  Word (r, c) sits at r * 32 + (c ^ s(r))
-// with s a bijection of the row bits (bit 0 -> 0, bits 1-2 -> 3-4, bits 3-4 -> 1-2): both the fragment writes and the
-// row reads touch 32 distinct banks.
-__device__ __forceinline__ int xpose_swz(int r) { return (r & 1) | ((r & 6) << 2) | ((r & 24) >> 2); }
+// Accumulator fragment -> one row half per thread.  A warp holds rows 16w .. 16w + 15 of the tile in one m64nBN
+// fragment: element 4j + e at (row lane/4, column 8j + 2(lane%4) + e), 4j + 2 + e at row lane/4 + 8.  acc_stage16<K>
+// writes columns 32K .. 32K + 31 into the warp's 16 x 32 fp32 block; lane l then reads row l & 15, columns
+// 16 (l >> 4) .. + 15.  Word (r, c) sits at r * 32 + (c ^ s(r)), s mapping row bits 0, 1, 2, 3 to bits 0, 3, 2 + 4, 1:
+// the fragment writes (8 rows x 4 column pairs) and the row reads (16 rows x 2 halves) each touch 32 distinct banks.
+__device__ __forceinline__ int xpose16_swz(int r) { return (r & 1) | ((r & 8) >> 2) | (r & 4) | ((r & 2) << 2) | ((r & 4) << 2); }
 template <int K, int S>
-__device__ __forceinline__ void acc_stage(const float (&a0)[S], const float (&a1)[S], float* buf, int lane) {
+__device__ __forceinline__ void acc_stage16(const float (&a)[S], float* buf, int lane) {
   const int r0 = lane >> 2, cl = 2 * (lane & 3);
 #pragma unroll
   for (int jj = 0; jj < 4; ++jj) {
@@ -291,20 +290,20 @@ __device__ __forceinline__ void acc_stage(const float (&a0)[S], const float (&a1
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
       const int c = 8 * jj + cl + e;
-      buf[r0 * 32 + (c ^ xpose_swz(r0))] = a0[4 * j + e];
-      buf[(r0 + 8) * 32 + (c ^ xpose_swz(r0 + 8))] = a0[4 * j + 2 + e];
-      buf[(r0 + 16) * 32 + (c ^ xpose_swz(r0 + 16))] = a1[4 * j + e];
-      buf[(r0 + 24) * 32 + (c ^ xpose_swz(r0 + 24))] = a1[4 * j + 2 + e];
+      buf[r0 * 32 + (c ^ xpose16_swz(r0))] = a[4 * j + e];
+      buf[(r0 + 8) * 32 + (c ^ xpose16_swz(r0 + 8))] = a[4 * j + 2 + e];
     }
   }
 }
-// runtime chunk index (uniform over the warp); register indices stay compile-time
-template <int S>
-__device__ __forceinline__ void acc_stage_k(int k, const float (&a0)[S], const float (&a1)[S], float* buf, int lane) {
-  if (k == 0) acc_stage<0>(a0, a1, buf, lane);
-  else if (S <= 32 || k == 1) acc_stage<1>(a0, a1, buf, lane);
-  else if (k == 2) acc_stage<S <= 32 ? 1 : 2>(a0, a1, buf, lane);
-  else acc_stage<S <= 32 ? 1 : 3>(a0, a1, buf, lane);
+// runtime chunk index (uniform over the warp, k < S / 16); register indices stay compile-time
+template <int S, int K = 0>
+__device__ __forceinline__ void acc_stage16_k(int k, const float (&a)[S], float* buf, int lane) {
+  if constexpr (K + 1 < S / 16) {
+    if (k == K) acc_stage16<K>(a, buf, lane);
+    else acc_stage16_k<S, K + 1>(k, a, buf, lane);
+  } else {
+    acc_stage16<K>(a, buf, lane);
+  }
 }
 // word j of this thread's staged row: rowp[j ^ s] (rowp = the 32-word row, s = its swizzle)
 template <int W>
@@ -312,11 +311,6 @@ __device__ __forceinline__ void acc_read_row(const float* rowp, int s, uint32_t 
 #pragma unroll
   for (int j = 0; j < W; ++j) v[j] = __float_as_uint(rowp[j ^ s]);
 }
-template <int W>
-__device__ __forceinline__ void acc_read(const float* buf, int lane, uint32_t (&v)[W]) {
-  acc_read_row<W>(buf + lane * 32, xpose_swz(lane), v);
-}
-
 
 // one W-column chunk starting at accumulator column cb of this thread's row (staged by the caller; read through
 // acc_read_row(rowp, sw))
@@ -345,19 +339,18 @@ __device__ __forceinline__ void epilogue_cols(const GemmDesc& d, const float* ro
   else epilogue_chunk<false, W, TAILN>(d, f, orow, ncol, lcol, nvalid, y2, xpre);
 }
 
-// The columns of this warpgroup's half of the tile, 32 at a time (a half of 16 mod 32 columns ends with a 16-column chunk).
+// The 32-column blocks of the tile that hold columns < N; each thread takes 16 columns of its row per block.
 template <int TAILN, int S>
-__device__ __forceinline__ void epilogue_row(const GemmDesc& d, const float (&a0)[S], const float (&a1)[S], float* buf,
-                                             int lane, int half, const TileCoord& c, int ocol0, long long orow, bool row_ok,
+__device__ __forceinline__ void epilogue_row(const GemmDesc& d, const float (&acc)[S], float* buf, int lane,
+                                             const TileCoord& c, int ocol0, long long orow, bool row_ok,
                                              float (&y2)[kMaxTail]) {
-  const int nh = d.block_n >> 1;
-  const float* rowp = buf + lane * 32;
-  const int sw = xpose_swz(lane);
-  for (int k = 0; 32 * k < nh; ++k) {
-    acc_stage_k(k, a0, a1, buf, lane);
+  const int r = lane & 15;
+  const float* rowp = buf + r * 32;
+  const int sw = xpose16_swz(r) ^ (lane & 16);     // column 16 (lane >> 4) + j of row r is word j ^ sw of rowp
+  for (int k = 0; 32 * k < 2 * S && c.n0 + 32 * k < d.N; ++k) {
+    acc_stage16_k(k, acc, buf, lane);
     __syncwarp();
-    if (32 * k + 32 <= nh) epilogue_cols<32, TAILN>(d, rowp, sw, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
-    else epilogue_cols<16, TAILN>(d, rowp, sw, half * nh + 32 * k, c, ocol0, orow, row_ok, y2);
+    epilogue_cols<16, TAILN>(d, rowp, sw, 32 * k + (lane & 16), c, ocol0, orow, row_ok, y2);
     __syncwarp();
   }
 }
@@ -365,7 +358,7 @@ __device__ __forceinline__ void epilogue_row(const GemmDesc& d, const float (&a0
 // ------------------------------------------------------------------------------------------------------------
 // Epilogue through shared memory + TMA (pf_gemm_kernel, d.tma_out != 0).
 // A thread owns one accumulator row, so direct global accesses are 32-byte pieces of 32 different rows per instruction:
-// one L2 request per sector.  Here each warp stages its 32 rows in a swizzled 4 KB tile and ONE elected lane moves it
+// one L2 request per sector.  Here each warp stages its 16 rows in a swizzled 2 KB tile and ONE elected lane moves it
 // with a bulk tensor copy: 128-byte requests, no LSU work; the fp32 residual stream is updated by a bulk reduce-add (no
 // read at all).  The staging tile doubles as the warp's transpose block, so the previous copy must have finished
 // reading it before the next accumulator block is staged.
@@ -376,138 +369,142 @@ struct EpiTma {
   uint8_t* stg_ptr;
 };
 
-// store this warp's 32 rows x 64 bf16 columns starting at column col
-__device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e, const TileCoord& c, int q, int col) {
+// store this warp's 16 rows x 128 B (64 bf16 / 32 fp32 columns) starting at column col
+__device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e, const TileCoord& c, int warp, int col) {
   if (d.a_mode == 1) {
-    const int r0 = q * 32;
+    const int r0 = warp * 16;
     const int yy = r0 / d.bw, xx = r0 - yy * d.bw;
     tma_store_4d(e.tm, e.stg_ptr, col, c.x0 + xx, c.y0 + yy, c.img);
   } else {
-    tma_store_2d(e.tm, e.stg_ptr, col, c.m0 + q * 32);
+    tma_store_2d(e.tm, e.stg_ptr, col, c.m0 + warp * 16);
   }
 }
 
-__device__ __forceinline__ void epi_act(const GemmDesc& d, float (&f)[32]) {
+__device__ __forceinline__ void epi_act(const GemmDesc& d, float (&f)[16]) {
   if (d.act == PF_ACT_RELU) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.0f);
+    for (int j = 0; j < 16; ++j) f[j] = fmaxf(f[j], 0.0f);
   } else if (d.act == PF_ACT_GELU) {
 #pragma unroll
-    for (int j = 0; j < 32; j += 2) gelu_erf2(f[j], f[j + 1]);
+    for (int j = 0; j < 16; j += 2) gelu_erf2(f[j], f[j + 1]);
   } else if (d.act == PF_ACT_SOFTPLUS) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) f[j] = softplus(f[j]);
+    for (int j = 0; j < 16; ++j) f[j] = softplus(f[j]);
   }
 }
-// acc + bias for 32 columns starting at logical column lcol (columns >= n_logical read no bias; TMA clips them)
-__device__ __forceinline__ void epi_bias(const GemmDesc& d, const uint32_t (&v)[32], int lcol, float (&f)[32]) {
+// acc + bias for 16 columns starting at logical column lcol (columns >= n_logical read no bias; TMA clips them)
+__device__ __forceinline__ void epi_bias(const GemmDesc& d, const uint32_t (&v)[16], int lcol, float (&f)[16]) {
 #pragma unroll
-  for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
+  for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
   if (d.bias == nullptr) return;
-  if (lcol + 32 <= d.n_logical) {
+  if (lcol + 16 <= d.n_logical) {
     const float4* bp = reinterpret_cast<const float4*>(d.bias + lcol);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
+    for (int j = 0; j < 4; ++j) {
       const float4 b = __ldg(bp + j);
       f[4 * j] += b.x; f[4 * j + 1] += b.y; f[4 * j + 2] += b.z; f[4 * j + 3] += b.w;
     }
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) if (lcol + j < d.n_logical) f[j] += __ldg(d.bias + lcol + j);
+    for (int j = 0; j < 16; ++j) if (lcol + j < d.n_logical) f[j] += __ldg(d.bias + lcol + j);
   }
 }
 
-// bf16 output: groups of 64 columns (128-byte row segments) of this warpgroup's half
+// bf16 output: groups of 64 columns (128-byte row segments).  Lane l holds row l & 15 and columns 16 (l >> 4) .. + 15
+// of both 32-column halves of a group, i.e. 16-byte pieces 2 (l >> 4) + {0, 1} and 4 + 2 (l >> 4) + {0, 1} of its row.
 template <int S>
-__device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&a0)[S],
-                                                       const float (&a1)[S], int half, const TileCoord& c, int q,
-                                                       int lane) {
-  const int nh = d.block_n >> 1;
+__device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
+                                                       const TileCoord& c, int warp, int lane) {
   float* buf = reinterpret_cast<float*>(e.stg_ptr);
-  for (int g = 0; 64 * g < nh; ++g) {
-    const int lcol = c.n0 + half * nh + g * 64;
+  const int r = lane & 15, h = lane >> 4;
+  const float* rowp = buf + r * 32;
+  const int sw = xpose16_swz(r) ^ (lane & 16);
+  for (int g = 0; 64 * g < 2 * S; ++g) {
+    const int lcol = c.n0 + g * 64;
     if (lcol >= d.n_logical) break;
     if (lane == 0) bulk_wait_read0();                      // the previous copy has finished reading the staging tile
     __syncwarp();
-    uint32_t v0[32], v1[32];
-    acc_stage_k(2 * g, a0, a1, buf, lane);
+    uint32_t v0[16], v1[16];
+    acc_stage16_k(2 * g, acc, buf, lane);
     __syncwarp();
-    acc_read<32>(buf, lane, v0);
+    acc_read_row<16>(rowp, sw, v0);
     __syncwarp();
-    acc_stage_k(2 * g + 1, a0, a1, buf, lane);
+    acc_stage16_k(2 * g + 1, acc, buf, lane);
     __syncwarp();
-    acc_read<32>(buf, lane, v1);
+    acc_read_row<16>(rowp, sw, v1);
     __syncwarp();
-    float f0[32], f1[32];
-    epi_bias(d, v0, lcol, f0);
-    epi_bias(d, v1, lcol + 32, f1);
+    float f0[16], f1[16];
+    epi_bias(d, v0, lcol + 16 * h, f0);
+    epi_bias(d, v1, lcol + 32 + 16 * h, f1);
     epi_act(d, f0);
     epi_act(d, f1);
-    const uint32_t row = e.stg + lane * 128;
-    const int sw = lane & 7;
+    const uint32_t row = e.stg + r * 128;
+    const int swz = r & 7;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      st_shared_v4(row + ((j ^ sw) << 4), pack_bf16(f0[8 * j], f0[8 * j + 1]), pack_bf16(f0[8 * j + 2], f0[8 * j + 3]),
+    for (int j = 0; j < 2; ++j) {
+      st_shared_v4(row + (((2 * h + j) ^ swz) << 4), pack_bf16(f0[8 * j], f0[8 * j + 1]), pack_bf16(f0[8 * j + 2], f0[8 * j + 3]),
                    pack_bf16(f0[8 * j + 4], f0[8 * j + 5]), pack_bf16(f0[8 * j + 6], f0[8 * j + 7]));
-      st_shared_v4(row + (((j + 4) ^ sw) << 4), pack_bf16(f1[8 * j], f1[8 * j + 1]), pack_bf16(f1[8 * j + 2], f1[8 * j + 3]),
+      st_shared_v4(row + (((4 + 2 * h + j) ^ swz) << 4), pack_bf16(f1[8 * j], f1[8 * j + 1]), pack_bf16(f1[8 * j + 2], f1[8 * j + 3]),
                    pack_bf16(f1[8 * j + 4], f1[8 * j + 5]), pack_bf16(f1[8 * j + 6], f1[8 * j + 7]));
     }
     fence_proxy_async_smem();
     __syncwarp();
-    if (lane == 0) { epi_tma_store(d, e, c, q, d.out_col0 + lcol); bulk_commit(); }
+    if (lane == 0) { epi_tma_store(d, e, c, warp, d.out_col0 + lcol); bulk_commit(); }
   }
 }
 
-// fp32 output (a_mode 0): chunks of 32 columns (128-byte row segments).  The residual-stream update x += gamma * (acc +
-// bias) stages gamma * (acc + bias) and lets the copy engine ADD it into x (cp.reduce.async.bulk.tensor .add.f32,
-// performed in the L2): the SM never reads x.  Each element is updated by exactly one tile: deterministic.
+// fp32 output (a_mode 0): chunks of 32 columns (128-byte row segments), lane l holding row l & 15, 16-byte pieces
+// 4 (l >> 4) .. + 3.  The residual-stream update x += gamma * (acc + bias) stages gamma * (acc + bias) and lets the copy
+// engine ADD it into x (cp.reduce.async.bulk.tensor .add.f32, performed in the L2): the SM never reads x.  Each element
+// is updated by exactly one tile: deterministic.
 template <int S>
-__device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma& e, const float (&a0)[S],
-                                                      const float (&a1)[S], int half, const TileCoord& c, int q,
-                                                      int lane) {
-  const int nh = d.block_n >> 1;
+__device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
+                                                      const TileCoord& c, int warp, int lane) {
   float* buf = reinterpret_cast<float*>(e.stg_ptr);
-  for (int ch = 0; 32 * ch < nh; ++ch) {
-    const int lcol = c.n0 + half * nh + ch * 32;
+  const int r = lane & 15, h = lane >> 4;
+  const float* rowp = buf + r * 32;
+  const int sw = xpose16_swz(r) ^ (lane & 16);
+  for (int ch = 0; 32 * ch < 2 * S; ++ch) {
+    const int lcol = c.n0 + ch * 32;
     if (lcol >= d.n_logical) break;
     if (lane == 0) bulk_wait_read0();                      // the previous copy has finished reading the staging tile
     __syncwarp();
-    uint32_t v[32];
-    acc_stage_k(ch, a0, a1, buf, lane);
+    uint32_t v[16];
+    acc_stage16_k(ch, acc, buf, lane);
     __syncwarp();
-    acc_read<32>(buf, lane, v);
+    acc_read_row<16>(rowp, sw, v);
     __syncwarp();
-    float f[32];
-    epi_bias(d, v, lcol, f);
+    const int l0 = lcol + 16 * h;
+    float f[16];
+    epi_bias(d, v, l0, f);
     epi_act(d, f);
     if (d.gamma != nullptr) {
-      if (lcol + 32 <= d.n_logical) {
+      if (l0 + 16 <= d.n_logical) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 g = __ldg(reinterpret_cast<const float4*>(d.gamma + lcol) + j);
+        for (int j = 0; j < 4; ++j) {
+          const float4 g = __ldg(reinterpret_cast<const float4*>(d.gamma + l0) + j);
           f[4 * j] *= g.x; f[4 * j + 1] *= g.y; f[4 * j + 2] *= g.z; f[4 * j + 3] *= g.w;
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) f[j] = lcol + j < d.n_logical ? f[j] * __ldg(d.gamma + lcol + j) : 0.f;
+        for (int j = 0; j < 16; ++j) f[j] = l0 + j < d.n_logical ? f[j] * __ldg(d.gamma + l0 + j) : 0.f;
       }
     }
-    const uint32_t row = e.stg + lane * 128;
-    const int sw = lane & 7;
+    const uint32_t row = e.stg + r * 128;
+    const int swz = r & 7;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      st_shared_v4(row + ((j ^ sw) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]),
+    for (int j = 0; j < 4; ++j)
+      st_shared_v4(row + (((4 * h + j) ^ swz) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]),
                    __float_as_uint(f[4 * j + 2]), __float_as_uint(f[4 * j + 3]));
     fence_proxy_async_smem();
     __syncwarp();
     if (lane == 0) {
-      if (d.gamma != nullptr) tma_reduce_add_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + q * 32);
-      else tma_store_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + q * 32);
+      if (d.gamma != nullptr) tma_reduce_add_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + warp * 16);
+      else tma_store_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + warp * 16);
       bulk_commit();
     }
   }
 }
-
 
 // Tile schedule.  Plain: CTA b takes tiles b, b + grid, ...  Multicast pairs (MC): cluster c takes tile PAIRS c, c + clusters, ...
 // where pair p = (m-tile pair p / n_tiles, n-tile p % n_tiles) and the CTA of cluster rank r owns m-tile 2 * mp + r
@@ -545,44 +542,42 @@ __device__ __forceinline__ void tail_store(const GemmDesc& d, long long orow, co
   }
 }
 
-// Epilogue of one tile by consumer warp `warp` (rows 32 (warp & 3) + lane, the columns of warpgroup warp >> 2).
+// Epilogue of one tile by consumer warp `warp`: tile rows 16 warp .. 16 warp + 15, all 2 S columns.  Lanes l and
+// l ^ 16 share row l & 15.  et == nullptr (halo kernel): direct stores only.
 template <int S>
-__device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord& c, const float (&a0)[S],
-                                              const float (&a1)[S], int warp, int lane, float* buf, float* tail_smem,
-                                              EpiTma* et) {
-  const int q = warp & 3;                 // 32-row slice of the tile owned by this warp
-  const int half = warp >> 2;             // warpgroup: which half of the N tile
-  const int r = q * 32 + lane;            // accumulator row owned by this thread
+__device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord& c, const float (&acc)[S], int warp,
+                                              int lane, float* buf, EpiTma* et) {
+  const int r = 16 * warp + (lane & 15);   // accumulator row of this thread
   // ---- row mapping
   bool row_ok;
   long long orow;       // output row (pixel / token) index
   if (d.a_mode == 1) {
-    int yy = r / d.bw, xx = r - yy * d.bw;
-    int y = c.y0 + yy, x = c.x0 + xx;
-    row_ok = (y < d.H) && (x < d.W) && (c.img < d.NB);     // img >= NB: the phantom tile that pairs an odd last m-tile
+    const int yy = r / d.bw, xx = r - yy * d.bw;
+    const int y = c.y0 + yy, x = c.x0 + xx;
+    row_ok = (y < d.H) && (x < d.W) && (c.img < d.NB);     // img >= NB: the phantom tile of a multicast cluster
     orow = (static_cast<long long>(c.img) * d.H + y) * d.W + x;
   } else {
-    int m = c.m0 + r;
+    const int m = c.m0 + r;
     row_ok = m < d.M;
     orow = m;
   }
   int ocol0 = c.n0;     // output column of accumulator column 0
   if (d.ps > 1 && d.a_mode == 0) {
     // ConvTranspose k==s: columns are ordered (ky, kx, cout); this N tile belongs to one (ky,kx).
-    int tap = c.n0 / d.ps_cout_pad;
+    const int tap = c.n0 / d.ps_cout_pad;
     ocol0 = c.n0 - tap * d.ps_cout_pad;
-    int ky = tap / d.ps, kx = tap - ky * d.ps;
-    int m = c.m0 + r;
-    int img = m / (d.H * d.W);
-    int rem = m - img * d.H * d.W;
-    int y = rem / d.W, x = rem - y * d.W;
+    const int ky = tap / d.ps, kx = tap - ky * d.ps;
+    const int m = c.m0 + r;
+    const int img = m / (d.H * d.W);
+    const int rem = m - img * d.H * d.W;
+    const int y = rem / d.W, x = rem - y * d.W;
     orow = (static_cast<long long>(img) * d.H * d.ps + y * d.ps + ky) * (d.W * d.ps) + x * d.ps + kx;
   }
   // TMA epilogue for this tile?  (the V^T tiles of the fused qkv projection keep the transposing direct store)
   const bool tma_tile = et != nullptr && d.tma_out != 0 && !(d.vt != nullptr && c.n0 >= d.vt_col0);
   if (tma_tile) {
-    if (d.tma_out == 1) epilogue_tile_tma_bf16(d, *et, a0, a1, half, c, q, lane);
-    else epilogue_tile_tma_f32(d, *et, a0, a1, half, c, q, lane);
+    if (d.tma_out == 1) epilogue_tile_tma_bf16(d, *et, acc, c, warp, lane);
+    else epilogue_tile_tma_f32(d, *et, acc, c, warp, lane);
     return;
   }
   // In pf_gemm_kernel `buf` is also this warp's TMA staging tile: a direct-store tile (the V^T tiles of the fused qkv
@@ -594,63 +589,19 @@ __device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord
   float y2[kMaxTail];
 #pragma unroll
   for (int i = 0; i < kMaxTail; ++i) y2[i] = 0.f;
-  if (d.w2 == nullptr) epilogue_row<0, S>(d, a0, a1, buf, lane, half, c, ocol0, orow, row_ok, y2);
-  else if (d.n2 <= 1) epilogue_row<1, S>(d, a0, a1, buf, lane, half, c, ocol0, orow, row_ok, y2);
-  else if (d.n2 <= 4) epilogue_row<4, S>(d, a0, a1, buf, lane, half, c, ocol0, orow, row_ok, y2);
-  else epilogue_row<kMaxTail, S>(d, a0, a1, buf, lane, half, c, ocol0, orow, row_ok, y2);
+  if (d.w2 == nullptr) epilogue_row<0>(d, acc, buf, lane, c, ocol0, orow, row_ok, y2);
+  else if (d.n2 <= 1) epilogue_row<1>(d, acc, buf, lane, c, ocol0, orow, row_ok, y2);
+  else if (d.n2 <= 4) epilogue_row<4>(d, acc, buf, lane, c, ocol0, orow, row_ok, y2);
+  else epilogue_row<kMaxTail>(d, acc, buf, lane, c, ocol0, orow, row_ok, y2);
   if (d.w2 != nullptr) {
-    // combine the two half-row partial sums of the fused trailing layer through shared memory
-    float* ts = tail_smem + r * kMaxTail;
-    if (half == 1) {
+    // lanes l and l ^ 16 hold the fused trailing layer's partial sums over alternate 16-column halves of one row
 #pragma unroll
-      for (int i = 0; i < kMaxTail; ++i) ts[i] = y2[i];
-    }
-    asm volatile("bar.sync %0, 64;" ::"r"(q + 1) : "memory");
-    if (half == 0) {
-#pragma unroll
-      for (int i = 0; i < kMaxTail; ++i) y2[i] += ts[i];
-    }
-    asm volatile("bar.sync %0, 64;" ::"r"(q + 1) : "memory");
+    for (int i = 0; i < kMaxTail; ++i)
+      if (i < d.n2) y2[i] += __shfl_xor_sync(0xffffffffu, y2[i], 16);
+    if (row_ok && lane < 16) tail_store(d, orow, y2);
   }
-  if (d.w2 != nullptr && row_ok && half == 0) tail_store(d, orow, y2);
 }
 
-// Columns warpgroup `half` issues for tile t: its share of tile_n_eff (a multiple of 16, possibly 0).
-__device__ __forceinline__ int half_n(const GemmDesc& d, int t, int half) {
-  const int nh = d.block_n >> 1;
-  const int n = tile_n_eff(d, t) - half * nh;
-  return n < 0 ? 0 : (n > nh ? nh : n);
-}
-
-// A fragments of the k16 steps k < nk of one 64-channel operand row block for this warp's two 16-row halves.  Row i of
-// half h is the tile row 32q + 16h + i; `rowaddr` gives its 128-byte shared-memory row (SWIZZLE_128B: 16-byte chunk j of
-// the row at address a sits at chunk j ^ ((a >> 7) & 7)).  Lane l addresses row l & 15, chunk 2k + (l >> 4).
-template <typename RowAddr>
-__device__ __forceinline__ void load_a_frags(RowAddr rowaddr, int q, int lane, int nk, uint32_t (&fa)[2][4][4]) {
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const uint32_t ra = rowaddr(32 * q + 16 * h + (lane & 15));
-    const uint32_t sw = (ra >> 7) & 7;
-#pragma unroll
-    for (int k = 0; k < kBlockK / 16; ++k)
-      if (k < nk) ldmatrix_x4(ra + (((2 * k + (lane >> 4)) ^ sw) << 4), fa[h][k]);
-  }
-}
-// wgmma over one operand block: both 16-row halves of every warp against this warpgroup's nw weight rows at bdesc
-template <int S>
-__device__ __forceinline__ void mma_block(float (&a0)[S], float (&a1)[S], const uint32_t (&fa)[2][4][4], uint64_t bdesc,
-                                          int nw, int nk, uint32_t accum) {
-  wgmma_fence();
-#pragma unroll
-  for (int k = 0; k < kBlockK / 16; ++k) {
-    if (k < nk) {
-      wgmma_rs_n(nw, a0, fa[0][k], bdesc + 2 * k, accum | k);
-      wgmma_rs_n(nw, a1, fa[1][k], bdesc + 2 * k, accum | k);
-    }
-  }
-  wgmma_commit();
-  wgmma_wait<0>();
-}
 // consumer warp done with a shared-memory stage: one arrival per warp, in every CTA of the cluster when the stage
 // was filled by multicast
 template <int CL>
@@ -670,19 +621,17 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
 
 // MC = true: launched as clusters of 2 CTAs that take two m-tiles of the SAME n-tile; each CTA fetches half of the
 // weight tile and multicasts it into both CTAs' shared memory (halves the weight traffic of the linear layers).
-template <bool MC, int S>
+template <bool MC, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_constant__ GemmKernelParams P) {
   constexpr int CL = MC ? 2 : 1;
+  constexpr int stage_bytes = gemm_stage_bytes(BN);
+  constexpr int stages = gemm_stages(BN);
   extern __shared__ uint8_t smem_raw[];
   const GemmDesc& d = P.d;
   // 1024-B alignment is required by SWIZZLE_128B operand tiles.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int stages = P.stages;
-  const int b_tile_bytes = d.block_n * kBlockK * 2;
-  const int stage_bytes = kATileBytes + b_tile_bytes;
-  uint8_t* epi_stage = smem + stages * stage_bytes;            // [kEpiWarps][4 KB], 1024-B aligned (stage sizes are 4 KB multiples)
-  float* tail_smem = reinterpret_cast<float*>(epi_stage + kEpiStageBytes);   // [128][kMaxTail]
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail_smem + 128 * kMaxTail);
+  uint8_t* xpose = smem + stages * stage_bytes;      // [kEpiWarps][2 KB], 1024-B aligned (stage sizes are 1 KB multiples)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kXposeWarp);
   uint64_t* empty_bar = full_bar + stages;
 
   const int warp = threadIdx.x >> 5;
@@ -724,7 +673,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
                 if (d.a_mode == 0) tma_load_2d(sa, &P.tmA[s], &full_bar[stage], ch * kBlockK, c.m0);
                 else tma_load_4d(sa, &P.tmA[s], &full_bar[stage], ch * kBlockK, c.x0 + dx, c.y0 + dy, c.img);
                 if (MC) {
-                  const int half_rows = d.block_n >> 1;
+                  constexpr int half_rows = BN / 2;
                   tma_load_2d_mc(sb + it.rank * half_rows * 128, &P.tmBh, &full_bar[stage], kb * kBlockK,
                                  c.n0 + it.rank * half_rows, static_cast<uint16_t>(3));
                 } else {
@@ -739,39 +688,37 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma mainloop + epilogue =====================
-    const int q = warp & 3, half = warp >> 2;
     EpiTma et;
-    et.tm = &P.tmOut; et.stg_ptr = epi_stage + warp * kStageTile; et.stg = smem_u32(et.stg_ptr);
+    et.tm = &P.tmOut; et.stg_ptr = xpose + warp * kXposeWarp; et.stg = smem_u32(et.stg_ptr);
     float* buf = reinterpret_cast<float*>(et.stg_ptr);
-    const uint32_t b_off = static_cast<uint32_t>(half * (d.block_n >> 1) * 128);
-    float a0[S], a1[S];
+    const uint32_t a_off = static_cast<uint32_t>((warp >> 2) * 64 * 128);   // this warpgroup's 64 rows of the A tile
+    float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
+    int rs = 0;                                             // oldest stage not yet released
     for (int ti = it.first; ti < it.count; ti += it.step) {
-      const int t = it.tile(ti);
-      const TileCoord c = decode_tile(d, t);
-      // the last n-tile issues only the columns that exist (rounded to 16): N = 544 runs as 192 + 192 + 160
-      const int nw = half_n(d, t, half);
+      const TileCoord c = decode_tile(d, it.tile(ti));
       uint32_t accum = 0;
-      for (int s = 0; s < d.num_src; ++s) {
-        const int nch = d.chunks[s];
-        const int nk_last = last_chunk_k16(d, s);        // K16 steps of the zero-padded last 64-channel chunk
-        for (int tap = 0; tap < d.taps; ++tap) {
-          for (int ch = 0; ch < nch; ++ch) {
-            const int nk = ch == nch - 1 ? nk_last : kBlockK / 16;
-            mbar_wait(&full_bar[stage], phase);
-            if (nw > 0) {
-              const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-              uint32_t fa[2][4][4];
-              load_a_frags([sa](int row) { return sa + row * 128; }, q, lane, nk, fa);
-              mma_block(a0, a1, fa, wgmma_desc_k128(sa + kATileBytes + b_off), nw, nk, accum);
-            }
-            accum = 1;
-            release_stage<CL>(&empty_bar[stage], lane);
-            if (++stage == stages) { stage = 0; phase ^= 1; }
-          }
+      for (int kb = 0; kb < P.k_steps; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+        const uint64_t adesc = wgmma_desc_k128(sa + a_off);
+        const uint64_t bdesc = wgmma_desc_k128(sa + kATileBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) Wgmma<BN>::ss(acc, adesc + 2 * k, bdesc + 2 * k, accum | k);
+        wgmma_commit();
+        accum = 1;
+        wgmma_wait<1>();                                    // the group of block kb - 1 is done ...
+        if (kb > 0) {                                       // ... and it was the last reader of its stage
+          release_stage<CL>(&empty_bar[rs], lane);
+          if (++rs == stages) rs = 0;
         }
+        if (++stage == stages) { stage = 0; phase ^= 1; }
       }
-      epilogue_tile(d, c, a0, a1, warp, lane, buf, tail_smem, &et);
+      wgmma_wait<0>();                                      // the tile's last block is done: its stage is free
+      release_stage<CL>(&empty_bar[rs], lane);
+      if (++rs == stages) rs = 0;
+      epilogue_tile(d, c, acc, warp, lane, buf, &et);
       __syncwarp();
     }
     if (lane == 0) bulk_wait0();    // the staging tiles are read (and the writes performed) before the CTA retires
@@ -801,11 +748,8 @@ constexpr int kHaloW = 10, kHaloH = 18;
 constexpr int kHaloBytes = kHaloW * kHaloH * 128;          // 23040
 constexpr int kHaloSlot = 24 * 1024;                        // 1024-B aligned slot
 constexpr int kHaloSlots = 3;
-constexpr int kMaxSmem = 227 * 1024;
-constexpr int kHaloXposeWarp = 16 * 32 * 4;                 // per consumer warp: 16 x 32 fp32 accumulator transpose
-constexpr int kHaloBarBytes = 512;
 // shared memory left for the weight ring next to the halo slots, transposes and barriers
-constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kHaloBarBytes - kEpiWarps * kHaloXposeWarp - kHaloSlots * kHaloSlot;
+constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kXposeWarp - kHaloSlots * kHaloSlot;
 // taps per weight stage: amortise the per-stage barrier round trip over several taps while two stages still fit
 __host__ __device__ constexpr int halo_kc(int bn) {
   return 2 * 9 * bn * kBlockK * 2 <= kHaloBBytes ? 9 : (2 * 3 * bn * kBlockK * 2 <= kHaloBBytes ? 3 : 1);
@@ -881,76 +825,6 @@ __device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&f
   for (int k = 0; k < kBlockK / 16; ++k) ldmatrix_x4(ra + (((2 * k + (lane >> 4)) ^ sw) << 4), fa[k]);
 }
 
-// Accumulator fragment -> one row half per thread.  A warp holds rows 16w .. 16w + 15 of the tile in one m64nBN
-// fragment: element 4j + e at (row lane/4, column 8j + 2(lane%4) + e), 4j + 2 + e at row lane/4 + 8.  acc_stage16<K>
-// writes columns 32K .. 32K + 31 into the warp's 16 x 32 fp32 block; lane l then reads row l & 15, columns
-// 16 (l >> 4) .. + 15.  Word (r, c) sits at r * 32 + (c ^ s(r)), s mapping row bits 0, 1, 2, 3 to bits 0, 3, 2 + 4, 1:
-// the fragment writes (8 rows x 4 column pairs) and the row reads (16 rows x 2 halves) each touch 32 distinct banks.
-__device__ __forceinline__ int xpose16_swz(int r) { return (r & 1) | ((r & 8) >> 2) | (r & 4) | ((r & 2) << 2) | ((r & 4) << 2); }
-template <int K, int S>
-__device__ __forceinline__ void acc_stage16(const float (&a)[S], float* buf, int lane) {
-  const int r0 = lane >> 2, cl = 2 * (lane & 3);
-#pragma unroll
-  for (int jj = 0; jj < 4; ++jj) {
-    const int j = 4 * K + jj;
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int c = 8 * jj + cl + e;
-      buf[r0 * 32 + (c ^ xpose16_swz(r0))] = a[4 * j + e];
-      buf[(r0 + 8) * 32 + (c ^ xpose16_swz(r0 + 8))] = a[4 * j + 2 + e];
-    }
-  }
-}
-// runtime chunk index (uniform over the warp, k < S / 16); register indices stay compile-time
-template <int S>
-__device__ __forceinline__ void acc_stage16_k(int k, const float (&a)[S], float* buf, int lane) {
-  constexpr int kLast = S / 16 - 1;
-  if (k == 0) acc_stage16<0>(a, buf, lane);
-  else if (k == 1) acc_stage16<(1 < kLast ? 1 : kLast)>(a, buf, lane);
-  else if (k == 2) acc_stage16<(2 < kLast ? 2 : kLast)>(a, buf, lane);
-  else if (k == 3) acc_stage16<(3 < kLast ? 3 : kLast)>(a, buf, lane);
-  else if (k == 4) acc_stage16<(4 < kLast ? 4 : kLast)>(a, buf, lane);
-  else acc_stage16<kLast>(a, buf, lane);
-}
-
-// The 32-column chunks of the tile that hold columns < N; each thread takes 16 columns of its row per chunk.
-template <int TAILN, int S>
-__device__ __forceinline__ void halo_epilogue_row(const GemmDesc& d, const float (&acc)[S], float* buf, int lane,
-                                                  const TileCoord& c, long long orow, bool row_ok, float (&y2)[kMaxTail]) {
-  const int r = lane & 15;
-  const float* rowp = buf + r * 32;
-  const int sw = xpose16_swz(r) ^ (lane & 16);     // column 16 (lane >> 4) + j of row r is word j ^ sw of rowp
-  for (int k = 0; 32 * k < 2 * S && c.n0 + 32 * k < d.N; ++k) {
-    acc_stage16_k(k, acc, buf, lane);
-    __syncwarp();
-    epilogue_cols<16, TAILN>(d, rowp, sw, 32 * k + (lane & 16), c, c.n0, orow, row_ok, y2);
-    __syncwarp();
-  }
-}
-
-template <int S>
-__device__ __forceinline__ void halo_epilogue_tile(const GemmDesc& d, const TileCoord& c, const float (&acc)[S], int warp,
-                                                   int lane, float* buf) {
-  const int r = 16 * warp + (lane & 15);           // tile row (bw = 8): pixel (r / 8, r % 8) of the 16 x 8 tile
-  const int y = c.y0 + (r >> 3), x = c.x0 + (r & 7);
-  const bool row_ok = (y < d.H) && (x < d.W) && (c.img < d.NB);   // img >= NB: phantom tile of a multicast cluster
-  const long long orow = (static_cast<long long>(c.img) * d.H + y) * d.W + x;
-  float y2[kMaxTail];
-#pragma unroll
-  for (int i = 0; i < kMaxTail; ++i) y2[i] = 0.f;
-  if (d.w2 == nullptr) halo_epilogue_row<0>(d, acc, buf, lane, c, orow, row_ok, y2);
-  else if (d.n2 <= 1) halo_epilogue_row<1>(d, acc, buf, lane, c, orow, row_ok, y2);
-  else if (d.n2 <= 4) halo_epilogue_row<4>(d, acc, buf, lane, c, orow, row_ok, y2);
-  else halo_epilogue_row<kMaxTail>(d, acc, buf, lane, c, orow, row_ok, y2);
-  if (d.w2 != nullptr) {
-    // lanes l and l ^ 16 hold the fused trailing layer's partial sums over alternate 16-column halves of one row
-#pragma unroll
-    for (int i = 0; i < kMaxTail; ++i)
-      if (i < d.n2) y2[i] += __shfl_xor_sync(0xffffffffu, y2[i], 16);
-    if (row_ok && lane < 16) tail_store(d, orow, y2);
-  }
-}
-
 // CL > 1: clusters of CL (2 or 4) CTAs take CL m-tiles (pixel tiles) of the SAME n-tile; each CTA fetches 1/CL of the rows
 // of every weight tile and multicasts it into all of them.  The weights are ~90 % of this kernel's L2 -> SM traffic (one
 // 23 KB halo against nine 4-24 KB tap tiles per 64-channel chunk).
@@ -967,7 +841,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_b = smem + kHaloSlots * kHaloSlot;
   uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][2 KB] accumulator transposes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kHaloXposeWarp);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kXposeWarp);
   uint64_t* a_full = bars;                                  // [kHaloSlots]
   uint64_t* a_empty = a_full + kHaloSlots;
   uint64_t* b_full = a_empty + kHaloSlots;                  // [stages]
@@ -1055,7 +929,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma over the nine shifted views of each halo tile + epilogue =====
-    float* buf = reinterpret_cast<float*>(xpose + warp * kHaloXposeWarp);
+    float* buf = reinterpret_cast<float*>(xpose + warp * kXposeWarp);
     const int arow = 16 * warp + (lane & 15);               // tile row this lane addresses for ldmatrix
     const uint32_t a_off = static_cast<uint32_t>(((arow >> 3) * kHaloW + (arow & 7)) * 128);
     float acc[BN / 2];
@@ -1099,7 +973,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
           if (++as == kHaloSlots) { as = 0; aph ^= 1; }
         }
       }
-      halo_epilogue_tile(d, c, acc, warp, lane, buf);
+      epilogue_tile(d, c, acc, warp, lane, buf, nullptr);
       __syncwarp();
     }
   }
@@ -1128,6 +1002,20 @@ static KernelFn halo_kernel_cl(int bn) {
 static KernelFn halo_kernel(int cl, int bn) {
   return cl == 4 ? halo_kernel_cl<4>(bn) : (cl == 2 ? halo_kernel_cl<2>(bn) : halo_kernel_cl<1>(bn));
 }
+// pf_gemm_kernel<MC, bn> for the widths of kGemmWidths, nullptr otherwise
+template <bool MC>
+static KernelFn gemm_kernel_mc(int bn) {
+  switch (bn) {
+    case 32: return pf_gemm_kernel<MC, 32>;
+    case 64: return pf_gemm_kernel<MC, 64>;
+    case 96: return pf_gemm_kernel<MC, 96>;
+    case 128: return pf_gemm_kernel<MC, 128>;
+    case 192: return pf_gemm_kernel<MC, 192>;
+    case 256: return pf_gemm_kernel<MC, 256>;
+    default: return nullptr;
+  }
+}
+static KernelFn gemm_kernel(bool mc, int bn) { return mc ? gemm_kernel_mc<true>(bn) : gemm_kernel_mc<false>(bn); }
 
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
                 const CUtensorMap* tmOut, cudaStream_t stream) {
@@ -1135,8 +1023,9 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   const int dev = current_device();
   if (!attr_done[dev]) {
     cudaError_t e = cudaSuccess;
-    for (KernelFn k : {pf_gemm_kernel<false, 32>, pf_gemm_kernel<false, 64>, pf_gemm_kernel<true, 32>, pf_gemm_kernel<true, 64>})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    for (bool mc : {false, true})
+      for (int bn : kGemmWidths)
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_kernel(mc, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (int cl : {1, 2, 4})
       for (int bn : {32, 64, 128, 192})
         if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
@@ -1145,9 +1034,6 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     attr_done[dev] = true;
   }
   const int g_sm_count = g_sm_counts[dev];
-  if (d.block_n % 32 != 0 || d.block_n < 32 || d.block_n > 256) return set_error("gemm: bad block_n %d", d.block_n);
-  // accumulator registers per fragment: 32 for half tiles of up to 64 columns, 64 above
-  const bool wide_acc = d.block_n > 128;
   {
     const long long rows = d.a_mode == 1 ? static_cast<long long>(d.NB) * d.H * d.W : d.M;
     int ktrue = 0;
@@ -1165,27 +1051,19 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   P.tmOut = tmOut ? *tmOut : tmB;
   P.d = d;
   if (d.tma_out && !tmOut) return set_error("gemm: tma_out without an output tensor map");
-  int stage_bytes = kATileBytes + d.block_n * kBlockK * 2;
-  int budget = kMaxSmem - 1024 /*align*/ - kEpiSmemBytes /*barriers, fused-tail scratch, transpose / staging blocks*/;
-  int stages = budget / stage_bytes;
-  if (stages > 8) stages = 8;
-  if (stages < 2) return set_error("gemm: not enough shared memory for 2 stages");
-  P.stages = stages;
   int ks = 0;
   for (int s = 0; s < d.num_src; ++s) ks += d.chunks[s] * d.taps;
   P.k_steps = ks;
   P.total_tiles = d.m_tiles * d.n_tiles;
   if (P.total_tiles <= 0 || ks <= 0) return set_error("gemm: empty problem");
   int grid = P.total_tiles < g_sm_count ? P.total_tiles : g_sm_count;
-  size_t smem = 1024 + static_cast<size_t>(stages) * stage_bytes + kEpiSmemBytes;
   if (d.halo) {
     const KernelFn hk = halo_kernel(d.halo_cl, d.block_n);
     if (hk == nullptr) return set_error("conv3 halo: block_n %d (32, 64, 128 or 192)", d.block_n);
     const int b_bytes = halo_kc(d.block_n) * d.block_n * kBlockK * 2;     // one weight stage
     const int hstages = halo_stages(d.block_n);
-    P.stages = hstages;
     size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * kHaloSlot + static_cast<size_t>(hstages) * b_bytes +
-                   kEpiWarps * kHaloXposeWarp + kHaloBarBytes;
+                   kEpiWarps * kXposeWarp + kBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
       // weight-multicast clusters of cl CTAs over (m-tile group, n-tile) work items.  Every CTA is persistent, so the grid
@@ -1217,24 +1095,29 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       le = launch_pdl(hk, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
     }
     if (le != cudaSuccess) return set_error("pf_conv3_halo_kernel launch: %s", cudaGetErrorString(le));
-  } else if (tmBh != nullptr) {
-    // weight-multicast pairs: clusters of 2 CTAs over (m-tile pair, n-tile) work items
-    const int pairs = ((d.m_tiles + 1) / 2) * d.n_tiles;
-    const int clusters = pairs < g_sm_count / 2 ? pairs : g_sm_count / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-    cudaLaunchAttribute at[2];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaError_t le = wide_acc ? cudaLaunchKernelEx(&cfg, pf_gemm_kernel<true, 64>, P) : cudaLaunchKernelEx(&cfg, pf_gemm_kernel<true, 32>, P);
-    if (le != cudaSuccess) return set_error("pf_gemm_kernel<multicast> launch: %s", cudaGetErrorString(le));
   } else {
-    cudaError_t le = wide_acc ? launch_pdl(pf_gemm_kernel<false, 64>, dim3(grid), dim3(kGemmThreads), smem, stream, P)
-                              : launch_pdl(pf_gemm_kernel<false, 32>, dim3(grid), dim3(kGemmThreads), smem, stream, P);
+    const KernelFn gk = gemm_kernel(tmBh != nullptr, d.block_n);
+    if (gk == nullptr) return set_error("gemm: block_n %d (32, 64, 96, 128, 192 or 256)", d.block_n);
+    const size_t smem = 1024 + static_cast<size_t>(gemm_stages(d.block_n)) * gemm_stage_bytes(d.block_n) +
+                        kEpiWarps * kXposeWarp + kBarBytes;
+    cudaError_t le;
+    if (tmBh != nullptr) {
+      // weight-multicast pairs: clusters of 2 CTAs over (m-tile pair, n-tile) work items
+      const int pairs = ((d.m_tiles + 1) / 2) * d.n_tiles;
+      const int clusters = pairs < g_sm_count / 2 ? pairs : g_sm_count / 2;
+      cudaLaunchConfig_t cfg = {};
+      cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+      cudaLaunchAttribute at[2];
+      at[0].id = cudaLaunchAttributeClusterDimension;
+      at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+      at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      at[1].val.programmaticStreamSerializationAllowed = 1;
+      cfg.attrs = at;
+      cfg.numAttrs = pdl_enabled() ? 2 : 1;
+      le = cudaLaunchKernelEx(&cfg, gk, P);
+    } else {
+      le = launch_pdl(gk, dim3(grid), dim3(kGemmThreads), smem, stream, P);
+    }
     if (le != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();

@@ -85,6 +85,10 @@ void count_launch(const char* name);
 void note_work(double flops, const char* fmt, ...);
 int check_launch(const char* what);
 
+// n-tile widths pf_gemm_kernel is compiled for (each consumer warpgroup holds a 64 x block_n fp32 accumulator tile in
+// registers)
+constexpr int kGemmWidths[] = {32, 64, 96, 128, 192, 256};
+
 // tmBh != nullptr selects the weight-multicast variant (clusters of 2 CTAs): a {64, block_n / 2} box map of the weights
 // tmOut: output tensor map when d.tma_out != 0
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
