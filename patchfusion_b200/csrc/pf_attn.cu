@@ -205,7 +205,8 @@ extern "C" int pf_attention(const void* qk, int32_t qk_ld, const void* vt, int32
   if (seq_pad < seq) return set_error("pf_attention: seq_pad %d < seq %d", seq_pad, seq);
   AttnParams P;
   if (tmap_3d_bf16(&P.tmQK, qk, 2 * D, seq, B, qk_ld, static_cast<uint64_t>(seq) * qk_ld, 64, 128, 1)) return 1;
-  // columns >= seq read as zeros (the padding of V^T is never touched)
+  // columns >= seq read as zeros: TMA zero-fills past the map's seq width, so the padding of V^T is never read
+  // (tests/test_gpu_attn_parity.py::test_layout_contracts fills it with NaN)
   if (tmap_2d_bf16(&P.tmVt, vt, seq, static_cast<uint64_t>(B) * heads * kHd, seq_pad, 64, 64)) return 1;
   P.B = B; P.seq = seq; P.heads = heads; P.D = D;
   P.n_qt = (seq + kQTile - 1) / kQTile;

@@ -251,7 +251,9 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
   bf16* att = static_cast<bf16*>(c.alloc(static_cast<size_t>(rows) * D * 2));
   bf16* hid = static_cast<bf16*>(c.alloc(static_cast<size_t>(rows) * 4 * D * 2));
   if (c.live() && seq_pad > seq) {
-    // V^T pad columns [seq, seq_pad) are read by the attention kernel's last KV tile (times P = 0): keep them finite
+    // V^T pad columns [seq, seq_pad): the attention kernel never reads them (its V^T tensor map is seq wide, so TMA
+    // zero-fills the last KV tile; tests/test_gpu_attn_parity.py runs it with NaN there).  Zeroed anyway as defence in
+    // depth: the qkv GEMM writes only columns < seq, and a NaN here would turn any future reader's P = 0 into NaN.
     cudaError_t e = cudaMemset2DAsync(vt + seq, static_cast<size_t>(seq_pad) * 2, 0, static_cast<size_t>(seq_pad - seq) * 2,
                                       static_cast<size_t>(B) * D, static_cast<cudaStream_t>(c.stream));
     if (e != cudaSuccess) c.chk(set_error("cudaMemset2DAsync(vt pad): %s", cudaGetErrorString(e)));

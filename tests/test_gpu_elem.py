@@ -26,6 +26,34 @@ def test_layernorm(cuda):
         check('layernorm %dx%d' % (rows, C), out, F.layer_norm(x, (C,), w, b, 1e-6), 1e-2)
 
 
+@pytest.mark.parametrize('C', [1024, 100])
+def test_layernorm_grouped(cuda, C):
+    """pf_layernorm_grouped as the ViT's last blocks use it: B images of seq tokens, the cls row dropped (skip 1),
+    npatch rows out per image.  x_ld and out_ld exceed C: NaN past C in x must not be read and the sentinel past C in
+    the output must survive, as must the rows past B * npatch.  C = 1024 is the largest row, C = 100 ends in a partial
+    group of 128 columns.  One token per image has mean 1e3 and std 1e-2: a one-pass E[x^2] - E[x]^2 variance
+    cancels to noise there, the two-pass one keeps it."""
+    import ctypes
+    from patchfusion_b200 import ops
+    g = _gen(7 + C)
+    B, seq = 3, 1037
+    npatch = seq - 1
+    x_ld, out_ld, sentinel = C + 12, C + 20, -1024.0
+    x = torch.full((B, seq, x_ld), float('nan'), device=cuda)
+    x[..., :C] = torch.randn(B, seq, C, device=cuda, generator=g) * 3 + 1
+    x[:, 5, :C] = 1e3 + 1e-2 * torch.randn(B, C, device=cuda, generator=g)
+    w, b = 1 + 0.5 * torch.randn(C, device=cuda, generator=g), torch.randn(C, device=cuda, generator=g)
+    out = torch.full((B * npatch + 8, out_ld), sentinel, dtype=torch.bfloat16, device=cuda)
+    ops.call('pf_layernorm_grouped', x, x_ld, w, b, ctypes.c_float(1e-6), B, seq, 1, npatch, C, out, out_ld,
+             ops.stream_ptr())
+    torch.cuda.synchronize()
+    ref = F.layer_norm(x[:, 1:, :C].double(), (C,), w.double(), b.double(), 1e-6).reshape(B * npatch, C)
+    check('layernorm grouped C%d' % C, out[:B * npatch, :C], ref, 1e-2)
+    o = out[:B * npatch, :C].view(B, npatch, C)
+    check('layernorm grouped C%d mean 1e3 std 1e-2' % C, o[:, 4], ref.view(B, npatch, C)[:, 4], 2e-2)
+    assert (out[:, C:] == sentinel).all() and (out[B * npatch:] == sentinel).all()
+
+
 def test_patch_im2col_and_tokens(cuda):
     from patchfusion_b200 import ops
     g = _gen(1)
