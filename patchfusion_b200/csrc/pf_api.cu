@@ -466,8 +466,11 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   const bool no_tma_epi = option(PF_OPT_TMA_EPILOGUE) == 0;
   CUtensorMap tmOut;
   d.tma_out = 0;
-  if (!no_tma_epi && !halo && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2) {
-    const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;     // columns >= N are clipped by the copy
+  // The copy clips columns >= out_col0 + N only at 16-byte granularity: a row that ends inside a 16-byte piece would get
+  // the staged zeros of columns N .. written over what the caller keeps there, so such outputs take the direct stores.
+  const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;
+  const bool ends16 = ocols % (d.out_f32 ? 4 : 8) == 0;
+  if (!no_tma_epi && !halo && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
     // each consumer warp stores its 16 rows in whole 64-column groups (bf16) / 32-column chunks (fp32)
     if (!d.out_f32 && bn % 64 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
       if (u->a_mode == 0) {
