@@ -1,5 +1,5 @@
-"""Model construction entry point with the reference's name (`build_model`).  Only the hot-path model type is
-registered in this build; anything else is reported with the list of what exists."""
+"""Model construction entry point with the reference's name (`build_model`).  Only the inference model types are
+registered in this build (PatchFusion, BaselinePretrain); anything else is reported with the list of what exists."""
 from estimator import registry
 
 

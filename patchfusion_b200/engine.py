@@ -48,14 +48,17 @@ class Map:
 
 
 class Engine:
-    def __init__(self, config, state_dict, device):
+    def __init__(self, config, state_dict, device, parts=('coarse', 'fine', 'fusion')):
+        """parts: the stages to pack and describe.  A single-branch model (BaselinePretrain) passes ('coarse',) or
+        ('fine',) with a state dict holding only that branch; the fusion stage reads the coarse and fine hparams."""
         self.cfg = config
+        self.parts = tuple(parts)
         self.dev = torch.device(device)
         self.P = tuple(_get(config, 'patch_process_shape'))
-        self.hp = {'coarse': branch_hparams(_get(config, 'coarse_branch')),
-                   'fine': branch_hparams(_get(config, 'fine_branch'))}
-        self.bcfg = {'coarse': _get(config, 'coarse_branch'), 'fine': _get(config, 'fine_branch')}
-        self.gf = guided_fusion_hparams(_get(config, 'guided_fusion'), self.P)
+        branches = [b for b in ('coarse', 'fine') if b in self.parts or 'fusion' in self.parts]
+        self.hp = {b: branch_hparams(_get(config, b + '_branch')) for b in branches}
+        self.bcfg = {b: _get(config, b + '_branch') for b in branches}
+        self.gf = guided_fusion_hparams(_get(config, 'guided_fusion'), self.P) if 'fusion' in self.parts else None
         self.bufs = {}
         self.arenas = {}
         self.generation = 0
@@ -67,8 +70,8 @@ class Engine:
         self.W = {}
         self._pack_all()
         self.sd = None   # fp32 originals are no longer needed on the device
-        self.c_branch = {'coarse': self._c_branch('coarse'), 'fine': self._c_branch('fine')}
-        self.c_fusion = self._c_fusion()
+        self.c_branch = {b: self._c_branch(b) for b in ('coarse', 'fine') if b in self.parts}
+        self.c_fusion = self._c_fusion() if 'fusion' in self.parts else None
 
     # ------------------------------------------------------------------ buffers
     def buf(self, key, shape, dtype=BF16):
@@ -221,9 +224,11 @@ class Engine:
         return Wd
 
     def _pack_all(self):
-        self.W['coarse'] = self._pack_branch('coarse')
-        self.W['fine'] = self._pack_branch('fine')
-        self.W['fusion'] = self._pack_fusion()
+        for b in ('coarse', 'fine'):
+            if b in self.parts:
+                self.W[b] = self._pack_branch(b)
+        if 'fusion' in self.parts:
+            self.W['fusion'] = self._pack_fusion()
         torch.cuda.synchronize(self.dev)
 
     # ------------------------------------------------------------------ C structs for the stage-level ABI

@@ -50,13 +50,27 @@ class AttrDict(dict):
 
 class Resize:
     """`model.resizer`: bilinear align_corners=True to patch_process_shape (depth_anything/transform.py:127-129 with
-    keep_aspect_ratio=False => always exactly (h, w), as used at patchfusion.py:94)."""
+    keep_aspect_ratio=False => always exactly (h, w), as used at patchfusion.py:94).
 
-    def __init__(self, width, height):
+    ensure_multiple_of > 1 (BaselinePretrain, baseline_pretrain.py:75,85): each side is rounded to the nearest
+    multiple, computed from the input size exactly as transform.py:56-57 / 111-113 do ('minimal', no aspect ratio
+    kept): (384, 512) -> 378 x 518, (392, 518) unchanged."""
+
+    def __init__(self, width, height, ensure_multiple_of=1):
         self.w, self.h = width, height
+        self.multiple = ensure_multiple_of
+
+    def out_size(self, height, width):
+        """(h, w) of the resized image for an input of height x width."""
+        if self.multiple == 1:
+            return int(self.h), int(self.w)
+        m = self.multiple
+        h = int(np.round(self.h / height * height / m) * m)
+        w = int(np.round(self.w / width * width / m) * m)
+        return h, w
 
     def __call__(self, x):
-        return nn.functional.interpolate(x, (int(self.h), int(self.w)), mode='bilinear', align_corners=True)
+        return nn.functional.interpolate(x, self.out_size(*x.shape[-2:]), mode='bilinear', align_corners=True)
 
 
 def _gauss_kernel(ksize, sigma):
@@ -89,7 +103,234 @@ def generatemask(size):
     return np.ascontiguousarray(m, dtype=np.float32)
 
 
-class PatchFusion(ParamTree, PyTorchModelHubMixin):
+class TiledModel(ParamTree):
+    """What `PatchFusion` and `BaselinePretrain` share, as the reference's `PatchFusion(BaselinePretrain)` does: tile
+    configuration, `make_lr`, blend masks, CUDA-graph replay, and the tiled forward of one image (regular passes
+    flattened into one ordered tile list, the random phase, the deterministic stitch and the tile sharding).  The
+    subclass supplies `compute(phase, img, geom, tiles, shard, plan)`: this rank's prediction block of the tile list."""
+
+    # pf_stitch_gather takes at most 4096 tiles per call: the random phase is computed and stitched in chunks of at
+    # most this many tiles, each continuing from the previous sums, so the canvas equals one pass bit for bit
+    random_chunk = 4096
+
+    def _runtime_init(self):
+        self._engine = None
+        self._graphs = {}
+        self.graph_launches = 0
+        self.use_cuda_graphs = os.environ.get('PF_B200_GRAPHS', '1') != '0'
+        self.partition = os.environ.get('PF_B200_PARTITION', 'greedy')
+        self._mask_cache = {}
+
+    def _hook_invalidate(self):
+        # sub-module loads (model.fine_branch.load_state_dict(sd), as the load_branch constructor path does) and
+        # .to()/.half() on a sub-module must drop the packed bf16 panels too: hook every container node
+        for m in self.modules():
+            if m is not self:
+                m.register_load_state_dict_post_hook(lambda mod, inc, _s=self: _s.invalidate())
+
+    def _init_constant_buffers(self, n_bins):
+        """constant buffers exactly as the reference constructs them"""
+        with torch.no_grad():
+            for name, buf in self.named_buffers():
+                if name.endswith('relative_position_index'):
+                    buf.copy_(relative_position_index())
+                elif name.endswith('k_idx'):
+                    buf.copy_(torch.arange(buf.numel()).view(buf.shape))
+                elif name.endswith('K_minus_1'):
+                    buf.fill_(float(n_bins - 1))
+                elif name.endswith('running_var'):
+                    buf.fill_(1.0)
+
+    # ------------------------------------------------------------------ reference API surface
+    def prepare_tile_cfg(self, image_raw_shape, patch_split_num):
+        assert image_raw_shape[0] % (2 * patch_split_num[0]) == 0, \
+            'image height should be divisible by 2 * patch_split_num[0]'
+        assert image_raw_shape[1] % (2 * patch_split_num[1]) == 0, \
+            'image width should be divisible by 2 * patch_split_num[1]'
+        pps = self.patch_process_shape
+        patch_reensemble_shape = (pps[0] * patch_split_num[0], pps[1] * patch_split_num[1])
+        patch_raw_shape = (image_raw_shape[0] // patch_split_num[0], image_raw_shape[1] // patch_split_num[1])
+        return {'patch_split_num': patch_split_num, 'patch_reensemble_shape': patch_reensemble_shape,
+                'patch_raw_shape': patch_raw_shape, 'image_raw_shape': image_raw_shape,
+                'raw_h_split_point': [int(patch_raw_shape[0] * i) for i in range(patch_split_num[0])],
+                'raw_w_split_point': [int(patch_raw_shape[1] * i) for i in range(patch_split_num[1])]}
+
+    def load_state_dict(self, *a, **kw):
+        self.invalidate()
+        return super().load_state_dict(*a, **kw)
+
+    def _apply(self, fn, *a, **kw):
+        self.invalidate()
+        return super()._apply(fn, *a, **kw)
+
+    @torch.no_grad()
+    def make_lr(self, image_hr):
+        """`image_lr = model.resizer(image)` of `tools/test_single_forward.py:13-14` on the device (same bilinear
+        align_corners=True resample, pf_crop_resize with one whole-image tile)."""
+        from . import ops
+        img = image_hr[0].float().contiguous()
+        H, W = img.shape[-2:]
+        ph, pw = self.resizer.out_size(H, W)
+        out = torch.empty((1, 3, ph, pw), dtype=torch.float32, device=img.device)
+        org = torch.zeros((1, 2), dtype=torch.int32, device=img.device)
+        ops.call('pf_crop_resize', img, H, W, org, 1, H, W, ph, pw, out, ops.stream_ptr())
+        return out
+
+    def _mask(self, size, device):
+        key = (tuple(size), str(device))
+        if key not in self._mask_cache:
+            self._mask_cache[key] = torch.tensor(generatemask(size) + 1e-3, device=device).contiguous()
+        return self._mask_cache[key]
+
+    # ------------------------------------------------------------------ tiling
+    def _graphed(self, key, fn):
+        """Run `fn` (a fixed kernel sequence over static buffers) through a CUDA graph: first call runs eagerly
+        (allocating the engine buffers and caching the TMA maps) and captures, later calls replay.  One graph per
+        (phase, micro-batch sizes, geometry): the ~2800 launches of a 4K P49 image collapse into one host call."""
+        from . import lib
+        if not self.use_cuda_graphs or lib.PROFILER is not None:
+            return fn()
+        ent = self._graphs.get(key)
+        eng = self._engine
+        if ent is None or ent[2] != eng.generation:     # workspaces were (re)allocated: old graphs point at freed memory
+            fn()
+            torch.cuda.synchronize()
+            g = torch.cuda.CUDAGraph()
+            n0 = lib.launch_count()
+            with torch.cuda.graph(g):
+                fn()
+            self._graphs[key] = (g, lib.launch_count() - n0, eng.generation)
+            return None
+        ent[0].replay()
+        self.graph_launches += ent[1]          # kernels executed by the replay (for bench.py's gpu_launches)
+        return None
+
+    def invalidate(self):
+        """Drop the packed-weight engine and the captured graphs (call after editing parameters in place; state-dict
+        loads and `.to()` on the model or any sub-module do it automatically)."""
+        self._engine, self._graphs = None, {}
+
+    def _micro_sizes(self, n, process_num):
+        nchunk = -(-n // process_num)
+        if self.partition == 'balanced':        # e.g. 49 tiles, process_num 9 -> 9,8,8,8,8,8
+            return [n // nchunk + (1 if i < n % nchunk else 0) for i in range(nchunk)]
+        return [min(process_num, n - i * process_num) for i in range(nchunk)]     # the reference's split (BP:293)
+
+    @staticmethod
+    def _chunks(n, size):
+        """[start, stop) ranges of the random phase's chunks: n tiles in order, at most `size` per chunk."""
+        return [(s, min(s + size, n)) for s in range(0, n, size)]
+
+    @staticmethod
+    def _check_shard(shard, group):
+        if shard is not None and shard[0] != 'emulate':
+            import torch.distributed as dist
+            assert dist.is_initialized() and dist.get_world_size(group) == shard[1] and dist.get_rank(group) == shard[0], \
+                'shard=(rank, world) must match the process group the blocks are gathered over'
+
+    def _exchange(self, compute, shard, group):
+        """The ONE collective of the tile-sharded path: all-gather of the per-rank prediction blocks.
+        shard=None: single device.  shard=('emulate', W): the W ranks are computed one after the other in this
+        process (test hook for 1-GPU boxes; same blocks, same stitch)."""
+        self._real_shard = shard is not None and shard[0] != 'emulate'
+        if shard is None:
+            return compute(None)
+        if shard[0] == 'emulate':
+            return torch.cat([compute((r, shard[1])).clone() for r in range(shard[1])])
+        from .parallel import gather_blocks
+        return gather_blocks(compute(shard), shard[1], group)
+
+    def _stitch_phase(self, eng, phase, full, origins, world, th, tw, mask, up, base, canvas, want, plan=None):
+        """pf_stitch_gather over the global tile list (deterministic order) -> requested canvases."""
+        from . import ops
+        from .parallel import slot_table
+        CH, CW = canvas
+        n = len(origins)
+        slots = slot_table(n, world, plan)
+        tab = eng.buf('stitch.tab.' + phase, (n, 3), torch.int32)
+        tab.copy_(torch.tensor([(oy, ox, sl) for (oy, ox), sl in zip(origins, slots)], dtype=torch.int32))
+        dev = full.device
+        outs = {k: torch.empty((CH, CW), dtype=torch.float32, device=dev) for k in want}
+        ops.call('pf_stitch_gather', full, tab, n, th, tw, mask, up[0], up[1],
+                 base[0] if base else None, base[1] if base else None, CH, CW,
+                 outs.get('num'), outs.get('den'), outs.get('avg'), ops.stream_ptr())
+        return outs
+
+    def _draw_random_boxes(self, n_calls, process_num, H, W, h, w, shard, group, dev):
+        """Random tile origins in the reference's draw order (baseline_pretrain.py:155-156: process_num rows, then ONE
+        shared column per call).  Under real sharding rank 0's draws are broadcast so every rank stitches the same
+        list (all ranks still advance their own `random` state identically)."""
+        boxes = []
+        for _ in range(n_calls):
+            ys = [random.randint(0, H - h - 1) for _ in range(process_num)]
+            x0 = random.randint(0, W - w - 1)
+            boxes += [(y, x0) for y in ys]
+        if shard is not None and shard[0] != 'emulate' and boxes:
+            import torch.distributed as dist
+            t = torch.tensor(boxes, dtype=torch.int32, device=dev if dist.get_backend(group) == 'nccl' else 'cpu')
+            dist.broadcast(t, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
+            boxes = [tuple(b) for b in t.cpu().tolist()]
+        return boxes
+
+    def _tiled_forward(self, eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_random_calls, compute,
+                       image_lr=None, plan_fn=None):
+        """Tiled inference of one image: the regular passes (baseline_pretrain.py:221-331, patchfusion.py:417-439) are
+        independent tiles whose stitch is a weighted sum, so all passes are flattened into one ordered tile list and
+        micro-batched; rN modes then resize the canvas to image_raw_shape and add `n_random_calls` calls of
+        `process_num` random tiles.  image_lr (PatchFusion) goes into its static buffer; plan_fn(n) gives the rank of
+        each regular tile (None: round-robin)."""
+        from . import ops
+        dev = image_hr.device
+        H, W = tile_cfg['image_raw_shape']
+        assert tuple(image_hr.shape[-2:]) == (H, W), 'image_hr must already be at image_raw_shape'
+        h, w = tile_cfg['patch_raw_shape']
+        ph, pw = self.patch_process_shape
+        RH, RW = tile_cfg['patch_reensemble_shape']
+        geom = (H, W, h, w, ph, pw)
+        world = 1 if shard is None else shard[1]
+        # inputs into static buffers (stable addresses for the captured graphs)
+        img = eng.buf('in.image_hr', (3, H, W), torch.float32)
+        img.copy_(image_hr[0])
+        if image_lr is not None:
+            eng.buf('in.image_lr', (1, 3, ph, pw), torch.float32).copy_(image_lr)
+        mask = self._mask((ph, pw), dev)
+        offsets = [((0, 0), (0, 0))]
+        if cai_mode == 'm2' or cai_mode[0] == 'r':
+            offsets += [((0, w // 2), (0, pw // 2)), ((h // 2, 0), (ph // 2, 0)), ((h // 2, w // 2), (ph // 2, pw // 2))]
+        raw, proc = [], []
+        for (oy, ox), (py, px) in offsets:
+            assert ox >= 0 and oy >= 0
+            ny, nx = (H - oy) // h, (W - ox) // w
+            raw += [(h * a + oy, w * b + ox) for a in range(ny) for b in range(nx)]
+            proc += [(ph * a + py, pw * b + px) for a in range(ny) for b in range(nx)]
+        is_r = cai_mode[0] == 'r'
+        plan = plan_fn(len(raw)) if plan_fn is not None else None
+        full = self._exchange(lambda sh: compute('reg', img, geom, raw, sh, plan), shard, group)
+        outs = self._stitch_phase(eng, 'reg', full, proc, world, ph, pw, mask, (0, 0), None, (RH, RW),
+                                  ('num', 'den') if is_r else ('avg',), plan)
+        if is_r:
+            n2 = torch.empty((H, W), dtype=torch.float32, device=dev)
+            d2 = torch.empty_like(n2)
+            ops.call('pf_stitch_resize', outs['num'], outs['den'], RH, RW, H, W, n2, d2, ops.stream_ptr())
+            boxes = self._draw_random_boxes(n_random_calls, process_num, H, W, h, w, shard, group, dev)
+            if boxes:
+                mask_r = self._mask((h, w), dev)
+                base = (n2, d2)
+                chunks = self._chunks(len(boxes), self.random_chunk)
+                for s0, s1 in chunks:
+                    part = boxes[s0:s1]
+                    last = s1 == len(boxes)
+                    full = self._exchange(lambda sh: compute('rnd', img, geom, part, sh, None), shard, group)
+                    outs = self._stitch_phase(eng, 'rnd', full, part, world, ph, pw, mask_r, (h, w), base, (H, W),
+                                              ('avg',) if last else ('num', 'den'))
+                    if not last:
+                        base = (outs['num'], outs['den'])
+            else:
+                outs = {'avg': n2 / d2}
+        return outs['avg'][None, None]
+
+
+class PatchFusion(TiledModel, PyTorchModelHubMixin):
     def __init__(self, config):
         nn.Module.__init__(self)
         if not isinstance(config, dict) and hasattr(config, 'to_dict'):
@@ -109,12 +350,8 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
         self.resizer = Resize(config.patch_process_shape[1], config.patch_process_shape[0])
         self._build_tree(state_layout(config))      # raises ValueError / NotImplementedError like the reference
         self.consistency_training = False
-        self._engine = None
-        self._graphs = {}
-        self.graph_launches = 0
+        self._runtime_init()
         self._coarse = None
-        self.use_cuda_graphs = os.environ.get('PF_B200_GRAPHS', '1') != '0'
-        self.partition = os.environ.get('PF_B200_PARTITION', 'greedy')
         # coarse branch + G2L (batch 1) on a side stream next to the first fine branch: measured in DESIGN.md
         self.overlap_coarse = os.environ.get('PF_B200_OVERLAP_COARSE', '1') != '0'
         self._side_stream = None
@@ -123,55 +360,19 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
         self.shard_coarse = os.environ.get('PF_B200_SHARD_COARSE', 'owner')
         self.owner_cost_tiles = float(os.environ.get('PF_B200_OWNER_COST', '2.7'))
         self._pack = None
-        self._mask_cache = {}
-        # sub-module loads (model.fine_branch.load_state_dict(sd), as the load_branch constructor path does) and
-        # .to()/.half() on a sub-module must drop the packed bf16 panels too: hook every container node
-        for m in self.modules():
-            if m is not self:
-                m.register_load_state_dict_post_hook(lambda mod, inc, _s=self: _s.invalidate())
+        self._hook_invalidate()
         if config.load_branch:
             for which, path in zip(('coarse_branch', 'fine_branch'), config.pretrain_model):
                 sd = torch.load(path, map_location='cpu')['model_state_dict']
                 getattr(self, which).load_state_dict(sd, strict=True)
-        # constant buffers exactly as the reference constructs them
-        with torch.no_grad():
-            for name, buf in self.named_buffers():
-                if name.endswith('relative_position_index'):
-                    buf.copy_(relative_position_index())
-                elif name.endswith('k_idx'):
-                    buf.copy_(torch.arange(buf.numel()).view(buf.shape))
-                elif name.endswith('K_minus_1'):
-                    buf.fill_(float(_get(config.coarse_branch, 'n_bins', 64) - 1))
-                elif name.endswith('running_var'):
-                    buf.fill_(1.0)
+        self._init_constant_buffers(_get(config.coarse_branch, 'n_bins', 64))
 
     # ------------------------------------------------------------------ reference API surface
-    def prepare_tile_cfg(self, image_raw_shape, patch_split_num):
-        assert image_raw_shape[0] % (2 * patch_split_num[0]) == 0, \
-            'image height should be divisible by 2 * patch_split_num[0]'
-        assert image_raw_shape[1] % (2 * patch_split_num[1]) == 0, \
-            'image width should be divisible by 2 * patch_split_num[1]'
-        pps = self.patch_process_shape
-        patch_reensemble_shape = (pps[0] * patch_split_num[0], pps[1] * patch_split_num[1])
-        patch_raw_shape = (image_raw_shape[0] // patch_split_num[0], image_raw_shape[1] // patch_split_num[1])
-        return {'patch_split_num': patch_split_num, 'patch_reensemble_shape': patch_reensemble_shape,
-                'patch_raw_shape': patch_raw_shape, 'image_raw_shape': image_raw_shape,
-                'raw_h_split_point': [int(patch_raw_shape[0] * i) for i in range(patch_split_num[0])],
-                'raw_w_split_point': [int(patch_raw_shape[1] * i) for i in range(patch_split_num[1])]}
-
     def load_dict(self, dict):
         return self.load_state_dict(dict, strict=False)
 
     def get_save_dict(self):
         return {k: v for k, v in self.state_dict().items() if 'coarse_branch' not in k and 'fine_branch' not in k}
-
-    def load_state_dict(self, *a, **kw):
-        self.invalidate()
-        return super().load_state_dict(*a, **kw)
-
-    def _apply(self, fn, *a, **kw):
-        self.invalidate()
-        return super()._apply(fn, *a, **kw)
 
     def init_synthetic_weights(self, seed=0):
         """Seeded random weights (no checkpoints are reachable offline)."""
@@ -189,24 +390,9 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
             self._engine = Engine(self.config, self.state_dict(), p.device)
         return self._engine
 
-    @torch.no_grad()
-    def make_lr(self, image_hr):
-        """`image_lr = model.resizer(image)` of `tools/test_single_forward.py:13-14` on the device (same bilinear
-        align_corners=True resample, pf_crop_resize with one whole-image tile)."""
-        from . import ops
-        img = image_hr[0].float().contiguous()
-        H, W = img.shape[-2:]
-        ph, pw = self.patch_process_shape
-        out = torch.empty((1, 3, ph, pw), dtype=torch.float32, device=img.device)
-        org = torch.zeros((1, 2), dtype=torch.int32, device=img.device)
-        ops.call('pf_crop_resize', img, H, W, org, 1, H, W, ph, pw, out, ops.stream_ptr())
-        return out
-
-    def _mask(self, size, device):
-        key = (tuple(size), str(device))
-        if key not in self._mask_cache:
-            self._mask_cache[key] = torch.tensor(generatemask(size) + 1e-3, device=device).contiguous()
-        return self._mask_cache[key]
+    def invalidate(self):
+        super().invalidate()
+        self._pack = None
 
     # ------------------------------------------------------------------ stage-level entry points (NCHW fp32 views)
     @staticmethod
@@ -268,33 +454,6 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
         return eng.fusion(crops, boxes, fd, ff, cd, cf, g2l)[:, None].clone()
 
     # ------------------------------------------------------------------ tiling
-    def _graphed(self, key, fn):
-        """Run `fn` (a fixed kernel sequence over static buffers) through a CUDA graph: first call runs eagerly
-        (allocating the engine buffers and caching the TMA maps) and captures, later calls replay.  One graph per
-        (phase, micro-batch sizes, geometry): the ~2800 launches of a 4K P49 image collapse into one host call."""
-        from . import lib
-        if not self.use_cuda_graphs or lib.PROFILER is not None:
-            return fn()
-        ent = self._graphs.get(key)
-        eng = self._engine
-        if ent is None or ent[2] != eng.generation:     # workspaces were (re)allocated: old graphs point at freed memory
-            fn()
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            n0 = lib.launch_count()
-            with torch.cuda.graph(g):
-                fn()
-            self._graphs[key] = (g, lib.launch_count() - n0, eng.generation)
-            return None
-        ent[0].replay()
-        self.graph_launches += ent[1]          # kernels executed by the replay (for bench.py's gpu_launches)
-        return None
-
-    def invalidate(self):
-        """Drop the packed-weight engine and the captured graphs (call after editing parameters in place; state-dict
-        loads and `.to()` on the model or any sub-module do it automatically)."""
-        self._engine, self._graphs, self._pack = None, {}, None
-
     def _coarse_stage(self, eng, lr, pack=False):
         """coarse branch + G2L of the whole image.  pack=True (tile-sharded owner): the results are copied into the
         contiguous pack buffer that is broadcast, and every later stage reads the pack."""
@@ -387,12 +546,6 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
             self._fusion_stage(eng, fine, io_box[s0:s0 + T], blk[s0:s0 + T])
             s0 += T
 
-    def _micro_sizes(self, n, process_num):
-        nchunk = -(-n // process_num)
-        if self.partition == 'balanced':        # e.g. 49 tiles, process_num 9 -> 9,8,8,8,8,8
-            return [n // nchunk + (1 if i < n % nchunk else 0) for i in range(nchunk)]
-        return [min(process_num, n - i * process_num) for i in range(nchunk)]     # the reference's split (BP:293)
-
     def _compute_phase(self, eng, phase, lr, img, geom, raw, process_num, shard, plan=None, group=None):
         """Fused predictions of this rank's tiles of the (global, ordered) tile list `raw` -> its block
         [block_rows, ph, pw] fp32 (row j = the j-th tile of the list that `plan` gives to this rank)."""
@@ -442,50 +595,6 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
         import torch.distributed as dist
         dist.broadcast(pack, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
 
-    def _exchange(self, compute, shard, group):
-        """The ONE collective of the tile-sharded path: all-gather of the per-rank prediction blocks.
-        shard=None: single device.  shard=('emulate', W): the W ranks are computed one after the other in this
-        process (test hook for 1-GPU boxes; same blocks, same stitch)."""
-        self._real_shard = shard is not None and shard[0] != 'emulate'
-        if shard is None:
-            return compute(None)
-        if shard[0] == 'emulate':
-            return torch.cat([compute((r, shard[1])).clone() for r in range(shard[1])])
-        from .parallel import gather_blocks
-        return gather_blocks(compute(shard), shard[1], group)
-
-    def _stitch_phase(self, eng, phase, full, origins, world, th, tw, mask, up, base, canvas, want, plan=None):
-        """pf_stitch_gather over the global tile list (deterministic order) -> requested canvases."""
-        from . import ops
-        from .parallel import slot_table
-        CH, CW = canvas
-        n = len(origins)
-        slots = slot_table(n, world, plan)
-        tab = eng.buf('stitch.tab.' + phase, (n, 3), torch.int32)
-        tab.copy_(torch.tensor([(oy, ox, sl) for (oy, ox), sl in zip(origins, slots)], dtype=torch.int32))
-        dev = full.device
-        outs = {k: torch.empty((CH, CW), dtype=torch.float32, device=dev) for k in want}
-        ops.call('pf_stitch_gather', full, tab, n, th, tw, mask, up[0], up[1],
-                 base[0] if base else None, base[1] if base else None, CH, CW,
-                 outs.get('num'), outs.get('den'), outs.get('avg'), ops.stream_ptr())
-        return outs
-
-    def _draw_random_boxes(self, n_calls, process_num, H, W, h, w, shard, group, dev):
-        """Random tile origins in the reference's draw order (baseline_pretrain.py:155-156: process_num rows, then ONE
-        shared column per call).  Under real sharding rank 0's draws are broadcast so every rank stitches the same
-        list (all ranks still advance their own `random` state identically)."""
-        boxes = []
-        for _ in range(n_calls):
-            ys = [random.randint(0, H - h - 1) for _ in range(process_num)]
-            x0 = random.randint(0, W - w - 1)
-            boxes += [(y, x0) for y in ys]
-        if shard is not None and shard[0] != 'emulate' and boxes:
-            import torch.distributed as dist
-            t = torch.tensor(boxes, dtype=torch.int32, device=dev if dist.get_backend(group) == 'nccl' else 'cpu')
-            dist.broadcast(t, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
-            boxes = [tuple(b) for b in t.cpu().tolist()]
-        return boxes
-
     @torch.no_grad()
     def forward(self, mode, image_lr, image_hr, depth_gt=None, crops_image_hr=None, crop_depths=None, bboxs=None,
                 tile_cfg=None, cai_mode='m1', process_num=4, shard=None, group=None):
@@ -500,58 +609,20 @@ class PatchFusion(ParamTree, PyTorchModelHubMixin):
         else:
             tile_cfg = self.prepare_tile_cfg(tile_cfg['image_raw_shape'], tile_cfg['patch_split_num'])
         assert image_hr.shape[0] == 1
-        if shard is not None and shard[0] != 'emulate':
-            import torch.distributed as dist
-            assert dist.is_initialized() and dist.get_world_size(group) == shard[1] and dist.get_rank(group) == shard[0], \
-                'shard=(rank, world) must match the process group the blocks are gathered over'
+        self._check_shard(shard, group)
         eng = self.engine()
-        dev = image_hr.device
-        H, W = tile_cfg['image_raw_shape']
-        assert tuple(image_hr.shape[-2:]) == (H, W), 'image_hr must already be at image_raw_shape'
-        h, w = tile_cfg['patch_raw_shape']
         ph, pw = self.patch_process_shape
-        RH, RW = tile_cfg['patch_reensemble_shape']
-        geom = (H, W, h, w, ph, pw)
-        world = 1 if shard is None else shard[1]
-        # inputs into static buffers (stable addresses for the captured graphs)
-        img = eng.buf('in.image_hr', (3, H, W), torch.float32)
-        img.copy_(image_hr[0])
-        lr = eng.buf('in.image_lr', (1, 3, ph, pw), torch.float32)
-        lr.copy_(image_lr)
-        mask = self._mask((ph, pw), dev)
-        offsets = [((0, 0), (0, 0))]
-        if cai_mode == 'm2' or cai_mode[0] == 'r':
-            offsets += [((0, w // 2), (0, pw // 2)), ((h // 2, 0), (ph // 2, 0)), ((h // 2, w // 2), (ph // 2, pw // 2))]
-        # The regular passes (baseline_pretrain.py:221-331, patchfusion.py:417-439) are independent tiles whose
-        # stitch is a weighted sum, so all passes are flattened into one ordered tile list and micro-batched.
-        raw, proc = [], []
-        for (oy, ox), (py, px) in offsets:
-            assert ox >= 0 and oy >= 0
-            ny, nx = (H - oy) // h, (W - ox) // w
-            raw += [(h * a + oy, w * b + ox) for a in range(ny) for b in range(nx)]
-            proc += [(ph * a + py, pw * b + px) for a in range(ny) for b in range(nx)]
-        is_r = cai_mode[0] == 'r'
-        plan = None
+        plan_fn = None
         if shard is not None and self.shard_coarse == 'owner':
             from .parallel import tile_plan
-            plan = tile_plan(len(raw), world, self.owner_cost_tiles)
-        full = self._exchange(lambda sh: self._compute_phase(eng, 'reg', lr, img, geom, raw, process_num, sh, plan, group),
-                              shard, group)
-        outs = self._stitch_phase(eng, 'reg', full, proc, world, ph, pw, mask, (0, 0), None, (RH, RW),
-                                  ('num', 'den') if is_r else ('avg',), plan)
-        if is_r:
-            from . import ops
-            n2 = torch.empty((H, W), dtype=torch.float32, device=dev)
-            d2 = torch.empty_like(n2)
-            ops.call('pf_stitch_resize', outs['num'], outs['den'], RH, RW, H, W, n2, d2, ops.stream_ptr())
-            boxes = self._draw_random_boxes(int(cai_mode[1:]) // process_num, process_num, H, W, h, w, shard, group, dev)
-            if boxes:
-                mask_r = self._mask((h, w), dev)
-                full = self._exchange(lambda sh: self._compute_phase(eng, 'rnd', lr, img, geom, boxes, process_num, sh),
-                                      shard, group)
-                outs = self._stitch_phase(eng, 'rnd', full, boxes, world, ph, pw, mask_r, (h, w), (n2, d2), (H, W),
-                                          ('avg',))
-            else:
-                outs = {'avg': n2 / d2}
-        depth = outs['avg'][None, None]
+            plan_fn = lambda n: tile_plan(n, shard[1], self.owner_cost_tiles)
+
+        def compute(phase, img, geom, tiles, sh, plan):
+            lr = eng.buf('in.image_lr', (1, 3, ph, pw), torch.float32)
+            return self._compute_phase(eng, phase, lr, img, geom, tiles, process_num, sh, plan, group)
+
+        # patchfusion.py:441-448: N // process_num calls of process_num random tiles
+        n_calls = int(cai_mode[1:]) // process_num if cai_mode[0] == 'r' else 0
+        depth = self._tiled_forward(eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_calls, compute,
+                                    image_lr=image_lr, plan_fn=plan_fn)
         return depth, {'rgb': image_lr, 'depth_pred': depth, 'depth_gt': depth_gt}

@@ -217,6 +217,14 @@ def state_layout(config):
     return L
 
 
+def branch_layout(branch_cfg, prefix):
+    """Layout of ONE branch (`BaselinePretrain` builds only the coarse or only the fine branch, BP:67-85): the keys of
+    `state_layout` under `prefix`, in the same order."""
+    L = OrderedDict()
+    _branch(L, prefix, branch_hparams(branch_cfg))
+    return L
+
+
 def relative_position_index(ws=WINDOW):
     """Swin relative-position lookup (`swin_layers.py:108-118`): index (i, j) -> row of the (2ws-1)^2 bias table."""
     ys, xs = torch.meshgrid(torch.arange(ws), torch.arange(ws), indexing='ij')
@@ -272,13 +280,16 @@ def _gain(key):
     raise AssertionError('no init rule for ' + key)
 
 
-def synthetic_state_dict(config, seed=0, dtype=torch.float32):
+def synthetic_state_dict(config, seed=0, dtype=torch.float32, prefix=''):
     """Seeded random weights with O(1) activations through the whole network.
 
     Linear/conv weights ~ N(0, gain/fan_in); the residual branches of the ViT/Swin blocks and the DPT RCUs are
     scaled down so the stream does not blow up; BN stats near identity; position tables small.  The values are a
     function of (key order, shapes, seed) only, so the GPU box regenerates exactly the weights the oracle and the
     golden fixtures were produced with.
+
+    prefix: keep only the keys under it (e.g. 'fine_branch.'), drawn from the same stream as the full dict, so a
+    single-branch model and a PatchFusion built from one seed hold identical branch weights.
     """
     g = torch.Generator().manual_seed(seed)
     layout = state_layout(config)
@@ -288,6 +299,8 @@ def synthetic_state_dict(config, seed=0, dtype=torch.float32):
         return torch.randn(shape, generator=g, dtype=torch.float32) * std
 
     for key, (shape, dt, kind) in layout.items():
+        if prefix and sd and not key.startswith(prefix):
+            break                                                # past the requested block: nothing left to keep
         leaf = key.split('.')[-1]
         if key.endswith('relative_position_index'):
             t = relative_position_index()
@@ -322,7 +335,8 @@ def synthetic_state_dict(config, seed=0, dtype=torch.float32):
             t = rn(shape, math.sqrt(_gain(key) / fan_in))
         else:
             raise AssertionError(key)
-        sd[key] = t.to(dt if dt != torch.float32 else dtype)
+        if key.startswith(prefix):
+            sd[key] = t.to(dt if dt != torch.float32 else dtype)
     return sd
 
 
