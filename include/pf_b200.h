@@ -147,6 +147,12 @@ int pf_resize_bilinear_f32(const float* in, int32_t B, int32_t H, int32_t W, int
 int pf_roi_crop_zoom(const void* feat, int32_t in_f32, int32_t h, int32_t w, int32_t C, int32_t in_ld,
                      const float* boxes, int32_t T, float spatial_scale, void* out, int32_t out_ld,
                      int32_t out_col0, void* stream);
+/* The same over a batch: feat is a [B,h,w,in_ld] map (fp32 when in_f32) and box t samples image tile_image[t]
+ * (int32 [T] on the device, values in [0, B); the batch column of the reference's bboxs_feat, patchfusion.py:240-257).
+ * tile_image == NULL reads image 0 for every box, i.e. pf_roi_crop_zoom. */
+int pf_roi_crop_zoom_batched(const void* feat, int32_t in_f32, int32_t h, int32_t w, int32_t C, int32_t in_ld,
+                             const int32_t* tile_image, const float* boxes, int32_t T, float spatial_scale, void* out,
+                             int32_t out_ld, int32_t out_col0, void* stream);
 /* nn.MaxPool2d(2) (guided_fusion_model.py:78) */
 int pf_maxpool2(const void* in, int32_t B, int32_t H, int32_t W, int32_t C, int32_t in_ld, void* out,
                 int32_t out_ld, void* stream);
@@ -158,6 +164,10 @@ int pf_im2col_3x3_s2(const void* in, int32_t B, int32_t H, int32_t W, int32_t C,
  * out_planar [T,3,ph,pw] fp32 (the tensor the reference hands to fine_forward). */
 int pf_crop_resize(const float* img, int32_t H, int32_t W, const int32_t* origins, int32_t T, int32_t th, int32_t tw,
                    int32_t ph, int32_t pw, float* out_planar, void* stream);
+/* The same from a batch of images [B,3,H,W]: tile t is cropped from image tile_image[t] (int32 [T] on the device,
+ * values in [0, B)), so one call may mix tiles of different images.  tile_image == NULL: image 0 (pf_crop_resize). */
+int pf_crop_resize_batched(const float* img, int32_t H, int32_t W, const int32_t* origins, const int32_t* tile_image,
+                           int32_t T, int32_t th, int32_t tw, int32_t ph, int32_t pw, float* out_planar, void* stream);
 /* U-Net input cat[coarse_depth_roi, fine_depth, rgb] (patchfusion.py:269) as NHWC bf16 with `ld` channels */
 int pf_pack_unet_input(const float* coarse_depth_roi, const float* fine_depth, const float* rgb_planar, int32_t T,
                        int32_t H, int32_t W, void* out, int32_t ld, void* stream);
@@ -205,6 +215,16 @@ int pf_window_attention(const void* qkv, const float* bias_table, int32_t Hp, in
                         int32_t shift, void* out, void* stream);
 /* x[H*W, C] += y[(padded grid), C] cropped (swin_layers.py:260-264); y fp32 */
 int pf_swin_residual_crop(float* x, const float* y, int32_t H, int32_t W, int32_t Wp, int32_t C, void* stream);
+/* Batched forms of the four ops above, one launch for B images: feat / x hold B maps of n = H*W rows back to back,
+ * the padded grids are [B, Hp*Wp, .] and the same ape is added to every image.  B = 1 is the single-image call. */
+int pf_g2l_embed_batched(const void* feat, int32_t feat_ld, const float* ape, int32_t B, int32_t n, int32_t C, float* x,
+                         void* stream);
+int pf_swin_norm_pad_batched(const float* x, const float* w, const float* b, float eps, int32_t B, int32_t H, int32_t W,
+                             int32_t Hp, int32_t Wp, int32_t C, void* out, void* stream);
+int pf_window_attention_batched(const void* qkv, const float* bias_table, int32_t B, int32_t Hp, int32_t Wp, int32_t C,
+                                int32_t heads, int32_t shift, void* out, void* stream);
+int pf_swin_residual_crop_batched(float* x, const float* y, int32_t B, int32_t H, int32_t W, int32_t Hp, int32_t Wp,
+                                  int32_t C, void* stream);
 
 /* ---- metric-bins tail (zoedepth_v1.py:173-219, attractor.py:164-208, dist_layers.py:36-121) -------------------- */
 /* x = emb + up(prev_emb) (attractor.py:175-178), NHWC bf16 */
@@ -349,6 +369,9 @@ size_t pf_branch_workspace_bytes(const pf_branch* w, int32_t B);
 /* images: planar fp32 [B,3,H,W] in [0,1], un-normalised.  out->depth [B,H,W] fp32 and the six taps live inside ws. */
 int pf_branch_forward(const pf_branch* w, const float* images, int32_t B, void* ws, size_t ws_bytes, pf_branch_out* out,
                       pf_tap_fn tap, void* tap_user, void* stream);
+/* coarse_feats: the six coarse maps of B whole images (every map's B must agree); out: the six G2L maps, batch B.
+ * Every op runs once over the batch (the GEMMs and LayerNorms over B*n rows), so a batch costs the launches of one
+ * image and image b equals its batch-1 result bit for bit. */
 size_t pf_g2l_workspace_bytes(const pf_fusion* w, const pf_map* coarse_feats);
 int pf_g2l_forward(const pf_fusion* w, const pf_map* coarse_feats, void* ws, size_t ws_bytes, pf_map* out,
                    void* stream);
@@ -359,6 +382,13 @@ int pf_fusion_forward(const pf_fusion* w, const float* crops, const float* boxes
                       const pf_map* fine_feats, const float* coarse_depth, const pf_map* coarse_feats,
                       const pf_map* g2l_maps, void* ws, size_t ws_bytes, float* depth_out, pf_tap_fn tap,
                       void* tap_user, void* stream);
+/* The same for tiles of several images: coarse_depth [B,H,W], coarse_feats and g2l_maps are batch-B maps and tile t
+ * reads image tile_image[t] of them (int32 [T] on the device, values in [0, B)).  tile_image == NULL: image 0 for
+ * every tile (pf_fusion_forward).  pf_fusion_workspace_bytes applies unchanged. */
+int pf_fusion_forward_batched(const pf_fusion* w, const float* crops, const float* boxes, const int32_t* tile_image,
+                              int32_t T, const float* fine_depth, const pf_map* fine_feats, const float* coarse_depth,
+                              const pf_map* coarse_feats, const pf_map* g2l_maps, void* ws, size_t ws_bytes,
+                              float* depth_out, pf_tap_fn tap, void* tap_user, void* stream);
 /* LayerNorm of rows [skip, skip + rows_out) of each group of rows_in rows (the patch tokens of every image, cls
  * dropped: vision_transformer.py:309-312): out row g*rows_out + i <- x row g*rows_in + skip + i */
 int pf_layernorm_grouped(const float* x, int32_t x_ld, const float* w, const float* b, float eps, int32_t groups,

@@ -118,23 +118,24 @@ class BaselinePretrain(TiledModel):
         return out[:, None].clone()
 
     # ------------------------------------------------------------------ fine target
-    def _tile_stage(self, eng, img, geom, sizes, io_raw, blk):
-        """crop+resize -> fine branch per micro-batch; the depth (in the reused tile arena) is copied into its rows
-        of the prediction block."""
+    def _tile_stage(self, eng, img, geom, sizes, io_raw, io_img, blk):
+        """crop+resize -> fine branch per micro-batch (a micro-batch may mix images: io_img gives each tile's, None =
+        image 0); the depth (in the reused tile arena) is copied into its rows of the prediction block."""
         from . import ops
         H, W, h, w, ph, pw = geom
         s0 = 0
         for T in sizes:
             crops = eng.buf('tile.crops', (T, 3, ph, pw), torch.float32)
-            ops.call('pf_crop_resize', img, H, W, io_raw[s0:s0 + T], T, h, w, ph, pw, crops, ops.stream_ptr())
+            ops.crop_resize(img, io_raw[s0:s0 + T], None if io_img is None else io_img[s0:s0 + T], h, w, ph, pw, crops)
             arena = eng.arena('tile', eng.branch_bytes('fine', T))
             fd, _ = eng.branch('fine', crops, ws=(arena, 0))
             blk[s0:s0 + T].copy_(fd)
             s0 += T
 
     def _compute_phase(self, eng, phase, img, geom, raw, process_num, shard):
-        """Fine-branch predictions of this rank's tiles of the ordered tile list `raw` -> its block
-        [block_rows, ph, pw] fp32 (round-robin: row j = tile rank + j * world)."""
+        """Fine-branch predictions of this rank's tiles of the ordered tile list `raw` ((image, y, x) items of img
+        [B,3,H,W], or (y, x) tiles of image 0) -> its block [block_rows, ph, pw] fp32 (round-robin: row j = tile
+        rank + j * world)."""
         from .parallel import shard_indices, block_rows
         H, W, h, w, ph, pw = geom
         rank, world = (0, 1) if shard is None else shard
@@ -143,19 +144,27 @@ class BaselinePretrain(TiledModel):
         blk = eng.buf('pred.blk.' + phase, (block_rows(n, world), ph, pw), torch.float32)
         if not own:
             return blk
+        chunk, images = self.split_tiles([raw[i] for i in own])
         io_raw = eng.buf('io.raw.' + phase, (len(own), 2), torch.int32)
-        io_raw.copy_(torch.tensor([raw[i] for i in own], dtype=torch.int32))
+        io_raw.copy_(torch.tensor(chunk, dtype=torch.int32))
+        B = img.shape[0] if img.dim() == 4 else 1
+        io_img = None
+        if B > 1:
+            io_img = eng.buf('io.img.' + phase, (len(own),), torch.int32)
+            io_img.copy_(torch.tensor(images, dtype=torch.int32))
         sizes = self._micro_sizes(len(own), process_num)
-        key = ('tiles', phase, tuple(sizes), blk.shape[0]) + tuple(geom)
-        self._graphed(key, lambda: self._tile_stage(eng, img, geom, sizes, io_raw, blk))
+        key = ('tiles', phase, tuple(sizes), blk.shape[0], B) + tuple(geom)
+        self._graphed(key, lambda: self._tile_stage(eng, img, geom, sizes, io_raw, io_img, blk))
         return blk
 
     @torch.no_grad()
     def forward(self, mode, image_lr, image_hr, depth_gt=None, crop_depths=None, crops_image_hr=None, bboxs=None,
                 tile_cfg=None, cai_mode='m1', process_num=4, shard=None, group=None):
         """BP:333-419 (mode='infer').  depth_gt defaults to None so `Tester.run` can drive this model.
-        Fine target only: `shard=(rank, world)` / `('emulate', W)` shards the tile list round-robin with one
-        all-gather before the deterministic stitch (as `PatchFusion.forward`)."""
+        Fine target: image_hr [B,3,H,W] with any B >= 1 (extension: the reference takes B = 1) -> [B,1,H',W']; the
+        tiles of all images are micro-batched together and image b equals the single-image call made after images
+        0..b-1 from the same `random` state.  `shard=(rank, world)` / `('emulate', W)` shards the tile list
+        round-robin with one all-gather before the deterministic stitch (as `PatchFusion.forward`)."""
         if mode == 'train':
             raise NotImplementedError('training is out of scope of the H100 hot-path build (SURVEY.md §2 rows 10,12)')
         if self.target == 'coarse':
@@ -167,7 +176,7 @@ class BaselinePretrain(TiledModel):
             tile_cfg = self.tile_cfg
         else:
             tile_cfg = self.prepare_tile_cfg(tile_cfg['image_raw_shape'], tile_cfg['patch_split_num'])
-        assert image_hr.shape[0] == 1
+        assert image_hr.shape[0] >= 1
         self._check_shard(shard, group)
         eng = self.engine()
 

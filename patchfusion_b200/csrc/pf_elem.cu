@@ -75,20 +75,22 @@ __global__ void layernorm_kernel(const float* __restrict__ x, int x_ld, const fl
   ln_row(x + src * x_ld, w, b, eps, C, out + static_cast<long long>(row) * out_ld, threadIdx.x & 31);
 }
 
-// LayerNorm into the zero-padded (Hp x Wp) Swin token grid.
+// LayerNorm into the zero-padded (Hp x Wp) Swin token grid, one grid per image of x[B, H*W, C].
 __global__ void swin_norm_pad_kernel(const float* __restrict__ x, const float* __restrict__ w,
-                                     const float* __restrict__ b, float eps, int H, int W, int Hp, int Wp, int C,
+                                     const float* __restrict__ b, float eps, int B, int H, int W, int Hp, int Wp, int C,
                                      bf16* __restrict__ out) {
-  int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  long long row = blockIdx.x * static_cast<long long>(blockDim.x >> 5) + (threadIdx.x >> 5);
   int lane = threadIdx.x & 31;
-  if (row >= Hp * Wp) return;
-  int y = row / Wp, xx = row - y * Wp;
-  bf16* orow = out + static_cast<long long>(row) * C;
+  if (row >= static_cast<long long>(B) * Hp * Wp) return;
+  const int img = static_cast<int>(row / (Hp * Wp));
+  const int r = static_cast<int>(row - static_cast<long long>(img) * Hp * Wp);
+  int y = r / Wp, xx = r - y * Wp;
+  bf16* orow = out + row * C;
   if (y >= H || xx >= W) {
     for (int c = lane * 4; c < C; c += 128) *reinterpret_cast<uint2*>(orow + c) = make_uint2(0u, 0u);
     return;
   }
-  ln_row(x + (static_cast<long long>(y) * W + xx) * C, w, b, eps, C, orow, lane);
+  ln_row(x + ((static_cast<long long>(img) * H + y) * W + xx) * C, w, b, eps, C, orow, lane);
 }
 
 // ------------------------------------------------------------------------------------------------ ViT input
@@ -335,14 +337,16 @@ __device__ __forceinline__ bool roi_coord(float c, int size, int& lo, int& hi, f
 }
 
 // grid: (ceil(w*cg / 256), h, T); thread = (output pixel x, 8-channel group [bf16] or channel [fp32]).
+// tile_image (nullable): box t samples image tile_image[t] of the [B, h, w, in_ld] map (NULL: image 0).
 template <bool F32>
 __global__ void roi_crop_zoom_kernel(const void* __restrict__ feat, int h, int w, int cg, int in_ld,
-                                     const float* __restrict__ boxes, float scale, void* __restrict__ out,
-                                     int out_ld, int out_col0) {
+                                     const int* __restrict__ tile_image, const float* __restrict__ boxes, float scale,
+                                     void* __restrict__ out, int out_ld, int out_col0) {
   const int tt = blockIdx.x * blockDim.x + threadIdx.x;
   if (tt >= w * cg) return;
   const int ox = tt / cg, g = tt - ox * cg;
   const int oy = blockIdx.y, t = blockIdx.z;
+  const size_t img = tile_image != nullptr ? static_cast<size_t>(__ldg(tile_image + t)) * h * w * in_ld : 0;
   const float x1 = __ldg(boxes + t * 4 + 0) * scale - 0.5f, y1 = __ldg(boxes + t * 4 + 1) * scale - 0.5f;
   const float x2 = __ldg(boxes + t * 4 + 2) * scale - 0.5f, y2 = __ldg(boxes + t * 4 + 3) * scale - 0.5f;
   const float bw = (x2 - x1) / w, bh = (y2 - y1) / h;
@@ -352,7 +356,7 @@ __global__ void roi_crop_zoom_kernel(const void* __restrict__ feat, int h, int w
   ok = roi_coord(sx, w, xl, xh, fx) && ok;
   const size_t p = (static_cast<size_t>(t) * h + oy) * w + ox;
   if (F32) {
-    const float* f = static_cast<const float*>(feat) + g;
+    const float* f = static_cast<const float*>(feat) + img + g;
     float v = 0.f;
     if (ok) {
       float v00 = f[(static_cast<size_t>(yl) * w + xl) * in_ld], v01 = f[(static_cast<size_t>(yl) * w + xh) * in_ld];
@@ -365,7 +369,7 @@ __global__ void roi_crop_zoom_kernel(const void* __restrict__ feat, int h, int w
 #pragma unroll
     for (int i = 0; i < 8; ++i) o[i] = 0.f;
     if (ok) {
-      const bf16* f = static_cast<const bf16*>(feat) + g * 8;
+      const bf16* f = static_cast<const bf16*>(feat) + img + g * 8;
       float a[8], bb[8], c[8], d[8];
       unpack8(__ldg(reinterpret_cast<const uint4*>(f + (static_cast<size_t>(yl) * w + xl) * in_ld)), a);
       unpack8(__ldg(reinterpret_cast<const uint4*>(f + (static_cast<size_t>(yl) * w + xh) * in_ld)), bb);
@@ -423,8 +427,10 @@ __global__ void im2col_3x3_s2_kernel(const bf16* __restrict__ in, int B, int H, 
   *reinterpret_cast<uint4*>(out + p * (9LL * C) + static_cast<long long>(tap) * C + g * 8) = v;
 }
 
-__global__ void crop_resize_kernel(const float* __restrict__ img, int H, int W, const int* __restrict__ origins, int T,
-                                   int th, int tw, int ph, int pw, float* __restrict__ out) {
+// tile_image (nullable): tile ti is cropped from image tile_image[ti] of img [B,3,H,W] (NULL: image 0).
+__global__ void crop_resize_kernel(const float* __restrict__ img, int H, int W, const int* __restrict__ origins,
+                                   const int* __restrict__ tile_image, int T, int th, int tw, int ph, int pw,
+                                   float* __restrict__ out) {
   long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
   long long total = static_cast<long long>(T) * 3 * ph * pw;
   if (idx >= total) return;
@@ -437,7 +443,8 @@ __global__ void crop_resize_kernel(const float* __restrict__ img, int H, int W, 
   int y0, y1, x0, x1; float fy, fx;
   ac_coord(oy, th, ph, y0, y1, fy);
   ac_coord(ox, tw, pw, x0, x1, fx);
-  const float* base = img + (static_cast<long long>(c) * H + origins[ti * 2]) * W + origins[ti * 2 + 1];
+  const long long plane = (tile_image != nullptr ? tile_image[ti] * 3LL : 0LL) + c;
+  const float* base = img + (plane * H + origins[ti * 2]) * W + origins[ti * 2 + 1];
   float v00 = base[static_cast<long long>(y0) * W + x0], v01 = base[static_cast<long long>(y0) * W + x1];
   float v10 = base[static_cast<long long>(y1) * W + x0], v11 = base[static_cast<long long>(y1) * W + x1];
   out[idx] = (1.f - fy) * ((1.f - fx) * v00 + fx * v01) + fy * ((1.f - fx) * v10 + fx * v11);
@@ -507,13 +514,15 @@ __global__ void depth_to_u16_kernel(const float* __restrict__ d, int H, int W, i
 }
 
 // ------------------------------------------------------------------------------------------------ Swin / G2L
-__global__ void g2l_embed_kernel(const bf16* __restrict__ feat, int feat_ld, const float* __restrict__ ape, int n, int C,
-                                 float* __restrict__ x) {
+// x[B, n, C] = feat rows + ape[n, C], the same embedding added to every image
+__global__ void g2l_embed_kernel(const bf16* __restrict__ feat, int feat_ld, const float* __restrict__ ape, int B, int n,
+                                 int C, float* __restrict__ x) {
   long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (idx >= static_cast<long long>(n) * C) return;
+  const long long per = static_cast<long long>(n) * C;
+  if (idx >= B * per) return;
   int c = static_cast<int>(idx % C);
   long long t = idx / C;
-  x[idx] = __bfloat162float(feat[t * feat_ld + c]) + ape[idx];
+  x[idx] = __bfloat162float(feat[t * feat_ld + c]) + ape[idx % per];
 }
 
 // One CTA per (window, head); thread i < 144 owns query row i.  K / V of the window live in shared memory as fp32
@@ -521,10 +530,13 @@ __global__ void g2l_embed_kernel(const bf16* __restrict__ feat, int feat_ld, con
 // shared-memory reads are broadcasts).  Scores are kept in the log2 domain (scale * log2e folded into q, log2e into
 // the bias table and the -100 shift mask) and the online softmax rescales only when the running maximum moves - one
 // ex2 per key instead of two exps and an unconditional rescale (r01: 4.7 ms per image in this kernel).
+// blockIdx.z = image: qkv / out hold B padded grids back to back.
 template <int HD>
 __global__ void __launch_bounds__(160) window_attention_kernel(const bf16* __restrict__ qkv,
                                                                const float* __restrict__ bias_table, int Hp, int Wp,
                                                                int C, int heads, int shift, bf16* __restrict__ out) {
+  qkv += static_cast<long long>(blockIdx.z) * Hp * Wp * (3 * C);
+  out += static_cast<long long>(blockIdx.z) * Hp * Wp * C;
   constexpr int WS = 12, NT = 144, HP = HD / 2;
   constexpr float kLog2e = 1.4426950408889634f;
   __shared__ uint64_t sk[NT][HP];
@@ -608,13 +620,17 @@ __global__ void __launch_bounds__(160) window_attention_kernel(const bf16* __res
   }
 }
 
-__global__ void swin_residual_crop_kernel(float* __restrict__ x, const float* __restrict__ y, int H, int W, int Wp, int C) {
+// x[B, H*W, C] += y[B, Hp*Wp, C] cropped to the top-left H x W of each padded grid
+__global__ void swin_residual_crop_kernel(float* __restrict__ x, const float* __restrict__ y, int B, int H, int W,
+                                          int Hp, int Wp, int C) {
   long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
-  if (idx >= static_cast<long long>(H) * W * C) return;
+  if (idx >= static_cast<long long>(B) * H * W * C) return;
   int c = static_cast<int>(idx % C);
   long long t = idx / C;
-  int xx = static_cast<int>(t % W), yy = static_cast<int>(t / W);
-  x[idx] += y[(static_cast<long long>(yy) * Wp + xx) * C + c];
+  int xx = static_cast<int>(t % W);
+  t /= W;
+  int yy = static_cast<int>(t % H), img = static_cast<int>(t / H);
+  x[idx] += y[((static_cast<long long>(img) * Hp + yy) * Wp + xx) * C + c];
 }
 
 // ------------------------------------------------------------------------------------------------ metric-bins tail
@@ -935,19 +951,26 @@ int pf_resize_bilinear_f32(const float* in, int32_t B, int32_t H, int32_t W, int
   return check_launch("resize_bilinear_f32_kernel");
 }
 
-int pf_roi_crop_zoom(const void* feat, int32_t in_f32, int32_t h, int32_t w, int32_t C, int32_t in_ld,
-                     const float* boxes, int32_t T, float spatial_scale, void* out, int32_t out_ld, int32_t out_col0,
-                     void* stream) {
+int pf_roi_crop_zoom_batched(const void* feat, int32_t in_f32, int32_t h, int32_t w, int32_t C, int32_t in_ld,
+                             const int32_t* tile_image, const float* boxes, int32_t T, float spatial_scale, void* out,
+                             int32_t out_ld, int32_t out_col0, void* stream) {
   if (in_f32) {
     dim3 grid(nblocks(static_cast<long long>(w) * C, 256), h, T);
-    roi_crop_zoom_kernel<true><<<grid, 256, 0, ST>>>(feat, h, w, C, in_ld, boxes, spatial_scale, out, out_ld, out_col0);
+    roi_crop_zoom_kernel<true><<<grid, 256, 0, ST>>>(feat, h, w, C, in_ld, tile_image, boxes, spatial_scale, out, out_ld,
+                                                     out_col0);
   } else {
     if (C % 8 || in_ld % 8 || out_ld % 8 || out_col0 % 8) return set_error("pf_roi_crop_zoom: channels/strides must be multiples of 8");
     dim3 grid(nblocks(static_cast<long long>(w) * (C / 8), 256), h, T);
-    roi_crop_zoom_kernel<false><<<grid, 256, 0, ST>>>(feat, h, w, C / 8, in_ld, boxes, spatial_scale, out, out_ld,
-                                                      out_col0);
+    roi_crop_zoom_kernel<false><<<grid, 256, 0, ST>>>(feat, h, w, C / 8, in_ld, tile_image, boxes, spatial_scale, out,
+                                                      out_ld, out_col0);
   }
   return check_launch("roi_crop_zoom_kernel");
+}
+
+int pf_roi_crop_zoom(const void* feat, int32_t in_f32, int32_t h, int32_t w, int32_t C, int32_t in_ld,
+                     const float* boxes, int32_t T, float spatial_scale, void* out, int32_t out_ld, int32_t out_col0,
+                     void* stream) {
+  return pf_roi_crop_zoom_batched(feat, in_f32, h, w, C, in_ld, nullptr, boxes, T, spatial_scale, out, out_ld, out_col0, stream);
 }
 
 int pf_maxpool2(const void* in, int32_t B, int32_t H, int32_t W, int32_t C, int32_t in_ld, void* out, int32_t out_ld,
@@ -968,11 +991,16 @@ int pf_im2col_3x3_s2(const void* in, int32_t B, int32_t H, int32_t W, int32_t C,
   return check_launch("im2col_3x3_s2_kernel");
 }
 
+int pf_crop_resize_batched(const float* img, int32_t H, int32_t W, const int32_t* origins, const int32_t* tile_image,
+                           int32_t T, int32_t th, int32_t tw, int32_t ph, int32_t pw, float* out_planar, void* stream) {
+  long long total = static_cast<long long>(T) * 3 * ph * pw;
+  crop_resize_kernel<<<nblocks(total, 256), 256, 0, ST>>>(img, H, W, origins, tile_image, T, th, tw, ph, pw, out_planar);
+  return check_launch("crop_resize_kernel");
+}
+
 int pf_crop_resize(const float* img, int32_t H, int32_t W, const int32_t* origins, int32_t T, int32_t th, int32_t tw,
                    int32_t ph, int32_t pw, float* out_planar, void* stream) {
-  long long total = static_cast<long long>(T) * 3 * ph * pw;
-  crop_resize_kernel<<<nblocks(total, 256), 256, 0, ST>>>(img, H, W, origins, T, th, tw, ph, pw, out_planar);
-  return check_launch("crop_resize_kernel");
+  return pf_crop_resize_batched(img, H, W, origins, nullptr, T, th, tw, ph, pw, out_planar, stream);
 }
 
 int pf_pack_unet_input(const float* coarse_depth_roi, const float* fine_depth, const float* rgb_planar, int32_t T,
@@ -998,24 +1026,42 @@ int pf_depth_to_u16(const float* depth, int32_t H, int32_t W, int32_t OH, int32_
   return check_launch("depth_to_u16_kernel");
 }
 
-int pf_g2l_embed(const void* feat, int32_t feat_ld, const float* ape, int32_t n, int32_t C, float* x, void* stream) {
-  g2l_embed_kernel<<<nblocks(static_cast<long long>(n) * C, 256), 256, 0, ST>>>(static_cast<const bf16*>(feat), feat_ld,
-                                                                                 ape, n, C, x);
+int pf_g2l_embed_batched(const void* feat, int32_t feat_ld, const float* ape, int32_t B, int32_t n, int32_t C, float* x,
+                         void* stream) {
+  if (B < 1) return set_error("pf_g2l_embed: B must be >= 1");
+  g2l_embed_kernel<<<nblocks(static_cast<long long>(B) * n * C, 256), 256, 0, ST>>>(static_cast<const bf16*>(feat),
+                                                                                     feat_ld, ape, B, n, C, x);
   return check_launch("g2l_embed_kernel");
+}
+
+int pf_g2l_embed(const void* feat, int32_t feat_ld, const float* ape, int32_t n, int32_t C, float* x, void* stream) {
+  return pf_g2l_embed_batched(feat, feat_ld, ape, 1, n, C, x, stream);
+}
+
+int pf_swin_norm_pad_batched(const float* x, const float* w, const float* b, float eps, int32_t B, int32_t H, int32_t W,
+                             int32_t Hp, int32_t Wp, int32_t C, void* out, void* stream) {
+  if (C % 4 || C > 1024) return set_error("pf_swin_norm_pad: C (<= 1024) must be a multiple of 4");
+  if (B < 1) return set_error("pf_swin_norm_pad: B must be >= 1");
+  swin_norm_pad_kernel<<<nblocks(static_cast<long long>(B) * Hp * Wp, 8), 256, 0, ST>>>(x, w, b, eps, B, H, W, Hp, Wp, C,
+                                                                                         static_cast<bf16*>(out));
+  return check_launch("swin_norm_pad_kernel");
 }
 
 int pf_swin_norm_pad(const float* x, const float* w, const float* b, float eps, int32_t H, int32_t W, int32_t Hp,
                      int32_t Wp, int32_t C, void* out, void* stream) {
-  if (C % 4 || C > 1024) return set_error("pf_swin_norm_pad: C (<= 1024) must be a multiple of 4");
-  swin_norm_pad_kernel<<<nblocks(static_cast<long long>(Hp) * Wp, 8), 256, 0, ST>>>(x, w, b, eps, H, W, Hp, Wp, C,
-                                                                                     static_cast<bf16*>(out));
-  return check_launch("swin_norm_pad_kernel");
+  return pf_swin_norm_pad_batched(x, w, b, eps, 1, H, W, Hp, Wp, C, out, stream);
 }
 
 int pf_window_attention(const void* qkv, const float* bias_table, int32_t Hp, int32_t Wp, int32_t C, int32_t heads,
                         int32_t shift, void* out, void* stream) {
+  return pf_window_attention_batched(qkv, bias_table, 1, Hp, Wp, C, heads, shift, out, stream);
+}
+
+int pf_window_attention_batched(const void* qkv, const float* bias_table, int32_t B, int32_t Hp, int32_t Wp, int32_t C,
+                                int32_t heads, int32_t shift, void* out, void* stream) {
   if (Hp % 12 || Wp % 12) return set_error("pf_window_attention: padded grid must be a multiple of the 12x12 window");
-  dim3 grid((Hp / 12) * (Wp / 12), heads);
+  if (B < 1 || B > 65535) return set_error("pf_window_attention: B must be in [1, 65535]");
+  dim3 grid((Hp / 12) * (Wp / 12), heads, B);
   const bf16* q = static_cast<const bf16*>(qkv);
   bf16* o = static_cast<bf16*>(out);
   switch (C / heads) {
@@ -1029,9 +1075,16 @@ int pf_window_attention(const void* qkv, const float* bias_table, int32_t Hp, in
   return check_launch("window_attention_kernel");
 }
 
-int pf_swin_residual_crop(float* x, const float* y, int32_t H, int32_t W, int32_t Wp, int32_t C, void* stream) {
-  swin_residual_crop_kernel<<<nblocks(static_cast<long long>(H) * W * C, 256), 256, 0, ST>>>(x, y, H, W, Wp, C);
+int pf_swin_residual_crop_batched(float* x, const float* y, int32_t B, int32_t H, int32_t W, int32_t Hp, int32_t Wp,
+                                  int32_t C, void* stream) {
+  if (B < 1) return set_error("pf_swin_residual_crop: B must be >= 1");
+  swin_residual_crop_kernel<<<nblocks(static_cast<long long>(B) * H * W * C, 256), 256, 0, ST>>>(x, y, B, H, W, Hp, Wp, C);
   return check_launch("swin_residual_crop_kernel");
+}
+
+int pf_swin_residual_crop(float* x, const float* y, int32_t H, int32_t W, int32_t Wp, int32_t C, void* stream) {
+  // one grid: its height never enters the address arithmetic
+  return pf_swin_residual_crop_batched(x, y, 1, H, W, H, Wp, C, stream);
 }
 
 int pf_add_upsampled(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, const void* prev, int32_t PH, int32_t PW,

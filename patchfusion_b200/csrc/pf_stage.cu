@@ -357,46 +357,52 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
 }
 
 // ---------------------------------------------------------------------------------------------------- G2L
+// B whole images at once (B = coarse[i].B): every op below is one launch over the batch.  Row-wise ops and GEMMs see
+// B*n (or B*Hp*Wp) rows, window attention and the pad / crop kernels take the image as a grid dimension.
 static void g2l_run(Ctx& c, const pf_fusion& Wf, const pf_map* coarse, pf_map* outs) {
   const int WS = 12;
+  const int B = coarse[0].B;
   for (int i = 0; i < 6; ++i) {
     const pf_g2l_level& L = Wf.g2l[i];
     const Map f = from_pf(coarse[i]);
     const int cc = L.C, h = f.H, w = f.W, n = h * w;
     const int Hp = (h + WS - 1) / WS * WS, Wp = (w + WS - 1) / WS * WS;
+    const long long rows = static_cast<long long>(B) * n, prow = static_cast<long long>(B) * Hp * Wp;
     if (!c.dry && L.ape_rows != n && !c.err)
       c.err = set_error("guided_fusion.num_patches[%d] = %d does not match the %dx%d coarse map", i, L.ape_rows, h, w);
-    float* x = static_cast<float*>(c.alloc(static_cast<size_t>(n) * cc * 4));
-    if (c.live()) c.chk(pf_g2l_embed(f.p, f.ld, L.ape, n, cc, x, c.stream));
-    bf16* npad = static_cast<bf16*>(c.alloc(static_cast<size_t>(Hp) * Wp * cc * 2));
-    bf16* qkv = static_cast<bf16*>(c.alloc(static_cast<size_t>(Hp) * Wp * 3 * cc * 2));
-    bf16* att = static_cast<bf16*>(c.alloc(static_cast<size_t>(Hp) * Wp * cc * 2));
-    float* prj = static_cast<float*>(c.alloc(static_cast<size_t>(Hp) * Wp * cc * 4));
-    bf16* hb = static_cast<bf16*>(c.alloc(static_cast<size_t>(n) * cc * 2));
-    bf16* hid = static_cast<bf16*>(c.alloc(static_cast<size_t>(n) * 4 * cc * 2));
+    if (f.B != B && !c.err) c.err = set_error("pf_g2l_forward: coarse map %d has batch %d, map 0 has %d", i, f.B, B);
+    float* x = static_cast<float*>(c.alloc(static_cast<size_t>(rows) * cc * 4));
+    if (c.live()) c.chk(pf_g2l_embed_batched(f.p, f.ld, L.ape, B, n, cc, x, c.stream));
+    bf16* npad = static_cast<bf16*>(c.alloc(static_cast<size_t>(prow) * cc * 2));
+    bf16* qkv = static_cast<bf16*>(c.alloc(static_cast<size_t>(prow) * 3 * cc * 2));
+    bf16* att = static_cast<bf16*>(c.alloc(static_cast<size_t>(prow) * cc * 2));
+    float* prj = static_cast<float*>(c.alloc(static_cast<size_t>(prow) * cc * 4));
+    bf16* hb = static_cast<bf16*>(c.alloc(static_cast<size_t>(rows) * cc * 2));
+    bf16* hid = static_cast<bf16*>(c.alloc(static_cast<size_t>(rows) * 4 * cc * 2));
     for (int b = 0; b < L.depth; ++b) {
       const pf_g2l_block& bw = L.blocks[b];
       const int shift = (b % 2 == 0) ? 0 : WS / 2;
-      if (c.live()) c.chk(pf_swin_norm_pad(x, bw.n1w, bw.n1b, 1e-5f, h, w, Hp, Wp, cc, npad, c.stream));
-      linear(c, bw.qkv, npad, static_cast<long long>(Hp) * Wp, cc, cc, qkv, 0, 3 * cc);
-      if (c.live()) c.chk(pf_window_attention(qkv, bw.table, Hp, Wp, cc, L.heads, shift, att, c.stream));
-      linear(c, bw.proj, att, static_cast<long long>(Hp) * Wp, cc, cc, prj, 1, cc);
-      if (c.live()) c.chk(pf_swin_residual_crop(x, prj, h, w, Wp, cc, c.stream));
-      if (c.live()) c.chk(pf_layernorm(x, cc, bw.n2w, bw.n2b, 1e-5f, n, cc, hb, cc, c.stream));
+      if (c.live()) c.chk(pf_swin_norm_pad_batched(x, bw.n1w, bw.n1b, 1e-5f, B, h, w, Hp, Wp, cc, npad, c.stream));
+      linear(c, bw.qkv, npad, prow, cc, cc, qkv, 0, 3 * cc);
+      if (c.live()) c.chk(pf_window_attention_batched(qkv, bw.table, B, Hp, Wp, cc, L.heads, shift, att, c.stream));
+      linear(c, bw.proj, att, prow, cc, cc, prj, 1, cc);
+      if (c.live()) c.chk(pf_swin_residual_crop_batched(x, prj, B, h, w, Hp, Wp, cc, c.stream));
+      if (c.live()) c.chk(pf_layernorm(x, cc, bw.n2w, bw.n2b, 1e-5f, static_cast<int32_t>(rows), cc, hb, cc, c.stream));
       GemmOpt g1; g1.act = PF_ACT_GELU;
-      linear(c, bw.fc1, hb, n, cc, cc, hid, 0, 4 * cc, g1);
+      linear(c, bw.fc1, hb, rows, cc, cc, hid, 0, 4 * cc, g1);
       GemmOpt g2; g2.gamma = L.ones;
-      linear(c, bw.fc2, hid, n, 4 * cc, 4 * cc, x, 1, cc, g2);
+      linear(c, bw.fc2, hid, rows, 4 * cc, 4 * cc, x, 1, cc, g2);
     }
-    Map o = c.map(1, h, w, cc);
-    if (c.live()) c.chk(pf_layernorm(x, cc, L.nw, L.nb, 1e-5f, n, cc, o.p, o.ld, c.stream));
+    Map o = c.map(B, h, w, cc);
+    if (c.live()) c.chk(pf_layernorm(x, cc, L.nw, L.nb, 1e-5f, static_cast<int32_t>(rows), cc, o.p, o.ld, c.stream));
     if (!c.dry && outs) outs[i] = to_pf(o);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------- fusion
-static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const float* boxes, int T,
-                       const float* fine_depth, const pf_map* fine_feats, const float* coarse_depth,
+// tile_image (nullable): tile t crops image tile_image[t] of the batch-B coarse depth, coarse maps and G2L maps
+static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const float* boxes, const int32_t* tile_image,
+                       int T, const float* fine_depth, const pf_map* fine_feats, const float* coarse_depth,
                        const pf_map* coarse_feats, const pf_map* g2l_maps, float* depth_out) {
   const int H = Wf.H, W = Wf.W;
   // ROI crop-zoom of the whole-image coarse maps + fused 3x3 convs with the fine maps (patchfusion.py:240-267)
@@ -406,13 +412,14 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
     const Map ff = from_pf(fine_feats[i]);
     Map roi = c.map(T, cf.H, cf.W, cf.C);
     if (c.live())
-      c.chk(pf_roi_crop_zoom(cf.p, 0, cf.H, cf.W, pad_to(cf.C, 8), cf.ld, boxes, T, static_cast<float>(cf.H) / H, roi.p,
-                             roi.ld, 0, c.stream));
+      c.chk(pf_roi_crop_zoom_batched(cf.p, 0, cf.H, cf.W, pad_to(cf.C, 8), cf.ld, tile_image, boxes, T,
+                                     static_cast<float>(cf.H) / H, roi.p, roi.ld, 0, c.stream));
     const Map* a[2] = {&roi, &ff};
     guide[i] = conv(c, Wf.fc[i], a, 2);
   }
   float* droi = static_cast<float*>(c.alloc(static_cast<size_t>(T) * H * W * 4));
-  if (c.live()) c.chk(pf_roi_crop_zoom(coarse_depth, 1, H, W, 1, 1, boxes, T, 1.0f, droi, 1, 0, c.stream));
+  if (c.live())
+    c.chk(pf_roi_crop_zoom_batched(coarse_depth, 1, H, W, 1, 1, tile_image, boxes, T, 1.0f, droi, 1, 0, c.stream));
   Map u = c.map(T, H, W, 5);
   if (c.live()) c.chk(pf_pack_unet_input(droi, fine_depth, crops, T, H, W, u.p, u.ld, c.stream));
   // encoder (guided_fusion_model.py:179-184)
@@ -443,7 +450,8 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
     }
     Map cr = c.map(T, h, w, gm.C);
     if (c.live())
-      c.chk(pf_roi_crop_zoom(gm.p, 0, h, w, pad_to(gm.C, 8), gm.ld, boxes, T, static_cast<float>(h) / H, cr.p, cr.ld, 0, c.stream));
+      c.chk(pf_roi_crop_zoom_batched(gm.p, 0, h, w, pad_to(gm.C, 8), gm.ld, tile_image, boxes, T, static_cast<float>(h) / H,
+                                     cr.p, cr.ld, 0, c.stream));
     const Map* a2[2] = {&e, &cr};
     Map y = conv_resampled(c, Wf.cv[i][0], a2, 2, h, w, gr);
     prev = conv1(c, Wf.cv[i][1], y, gr);
@@ -503,21 +511,29 @@ size_t pf_fusion_workspace_bytes(const pf_fusion* w, int32_t T, const pf_map* g2
   // shapes only: the fine / coarse maps share the G2L maps' geometry and channel counts
   pf_map fine[6];
   for (int i = 0; i < 6; ++i) { fine[i] = g2l_maps[i]; fine[i].B = T; fine[i].ptr = nullptr; }
-  fusion_run(c, *w, nullptr, nullptr, T, nullptr, fine, nullptr, g2l_maps, g2l_maps, nullptr);
+  fusion_run(c, *w, nullptr, nullptr, nullptr, T, nullptr, fine, nullptr, g2l_maps, g2l_maps, nullptr);
   return c.off + 256;
+}
+
+int pf_fusion_forward_batched(const pf_fusion* w, const float* crops, const float* boxes, const int32_t* tile_image,
+                              int32_t T, const float* fine_depth, const pf_map* fine_feats, const float* coarse_depth,
+                              const pf_map* coarse_feats, const pf_map* g2l_maps, void* ws, size_t ws_bytes,
+                              float* depth_out, pf_tap_fn tap, void* tap_user, void* stream) {
+  if (!w || !crops || !boxes || !fine_depth || !fine_feats || !coarse_depth || !coarse_feats || !g2l_maps || !ws ||
+      !depth_out || T < 1)
+    return set_error("pf_fusion_forward: null argument");
+  if (reinterpret_cast<uintptr_t>(ws) & 255) return set_error("pf_fusion_forward: workspace must be 256-byte aligned");
+  Ctx c = make_ctx(ws, ws_bytes, false, stream, tap, tap_user);
+  fusion_run(c, *w, crops, boxes, tile_image, T, fine_depth, fine_feats, coarse_depth, coarse_feats, g2l_maps, depth_out);
+  return c.err;
 }
 
 int pf_fusion_forward(const pf_fusion* w, const float* crops, const float* boxes, int32_t T, const float* fine_depth,
                       const pf_map* fine_feats, const float* coarse_depth, const pf_map* coarse_feats,
                       const pf_map* g2l_maps, void* ws, size_t ws_bytes, float* depth_out, pf_tap_fn tap,
                       void* tap_user, void* stream) {
-  if (!w || !crops || !boxes || !fine_depth || !fine_feats || !coarse_depth || !coarse_feats || !g2l_maps || !ws ||
-      !depth_out || T < 1)
-    return set_error("pf_fusion_forward: null argument");
-  if (reinterpret_cast<uintptr_t>(ws) & 255) return set_error("pf_fusion_forward: workspace must be 256-byte aligned");
-  Ctx c = make_ctx(ws, ws_bytes, false, stream, tap, tap_user);
-  fusion_run(c, *w, crops, boxes, T, fine_depth, fine_feats, coarse_depth, coarse_feats, g2l_maps, depth_out);
-  return c.err;
+  return pf_fusion_forward_batched(w, crops, boxes, nullptr, T, fine_depth, fine_feats, coarse_depth, coarse_feats,
+                                   g2l_maps, ws, ws_bytes, depth_out, tap, tap_user, stream);
 }
 
 }  // extern "C"

@@ -383,7 +383,8 @@ class Engine:
         return arr
 
     def g2l(self, coarse_feats):
-        """The six tile-invariant G2L maps of the whole-image coarse taps (computed once per image)."""
+        """The six tile-invariant G2L maps of the whole-image coarse taps (computed once per image).  The maps may hold
+        a batch of B images: one call then computes the B images' maps, batch B out."""
         from . import stage
         cm = self._pf_maps(coarse_feats)
         need = stage.g2l_workspace_bytes(self.c_fusion, cm)
@@ -396,8 +397,10 @@ class Engine:
         return stage.fusion_workspace_bytes(self.c_fusion, T, self._pf_maps(g2l_maps))
 
     def fusion(self, crops, boxes, fine_depth, fine_feats, coarse_depth, coarse_feats, g2l_maps, taps=None,
-               depth_out=None, ws=None):
-        """crops planar fp32 [T,3,H,W]; boxes fp32 [T,4] (device, patch_process units); returns fp32 [T,H,W]."""
+               depth_out=None, ws=None, tile_image=None):
+        """crops planar fp32 [T,3,H,W]; boxes fp32 [T,4] (device, patch_process units); returns fp32 [T,H,W].
+        tile_image (int32 [T] device tensor): tile t reads image tile_image[t] of the batch-B coarse depth [B,H,W],
+        coarse maps and G2L maps; None reads image 0 (the single-image call)."""
         from . import stage
         T = crops.shape[0]
         H, W = self.P
@@ -413,9 +416,12 @@ class Engine:
         assert depth_out.dtype == F32 and depth_out.is_contiguous() and tuple(depth_out.shape) == (T, H, W)
         for t_ in (crops, boxes, fine_depth, coarse_depth):
             assert t_.dtype == F32 and t_.is_contiguous()
+        if tile_image is not None:
+            assert tile_image.dtype == torch.int32 and tile_image.is_contiguous() and tile_image.numel() == T
         tap = self._tap_cb(arena, taps) if taps is not None else None
         stage.fusion_forward(self.c_fusion, crops, boxes, T, fine_depth, self._pf_maps(fine_feats), coarse_depth,
-                             self._pf_maps(coarse_feats), gm, arena.data_ptr() + off, need, depth_out, tap)
+                             self._pf_maps(coarse_feats), gm, arena.data_ptr() + off, need, depth_out, tap,
+                             tile_image=tile_image)
         if taps is not None:
             for i in range(6):
                 m = g2l_maps[i]

@@ -60,9 +60,11 @@ SIGNATURES = {
     'pf_resize_bilinear': [_p, _i, _i, _i, _i, _i, _i, _i, _p, _i, _i, _p],
     'pf_resize_bilinear_f32': [_p, _i, _i, _i, _i, _i, _i, _p, _p],
     'pf_roi_crop_zoom': [_p, _i, _i, _i, _i, _i, _p, _i, _f, _p, _i, _i, _p],
+    'pf_roi_crop_zoom_batched': [_p, _i, _i, _i, _i, _i, _p, _p, _i, _f, _p, _i, _i, _p],
     'pf_maxpool2': [_p, _i, _i, _i, _i, _i, _p, _i, _p],
     'pf_im2col_3x3_s2': [_p, _i, _i, _i, _i, _i, _p, _p],
     'pf_crop_resize': [_p, _i, _i, _p, _i, _i, _i, _i, _i, _p, _p],
+    'pf_crop_resize_batched': [_p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p],
     'pf_pack_unet_input': [_p, _p, _p, _i, _i, _i, _p, _i, _p],
     'pf_f32_to_bf16': [_p, _ll, _p, _p],
     'pf_ingest_u8': [_p, _i, _i, _i, _i, _i, _p, _p],
@@ -73,6 +75,10 @@ SIGNATURES = {
     'pf_swin_norm_pad': [_p, _p, _p, _f, _i, _i, _i, _i, _i, _p, _p],
     'pf_window_attention': [_p, _p, _i, _i, _i, _i, _i, _p, _p],
     'pf_swin_residual_crop': [_p, _p, _i, _i, _i, _i, _p],
+    'pf_g2l_embed_batched': [_p, _i, _p, _i, _i, _i, _p, _p],
+    'pf_swin_norm_pad_batched': [_p, _p, _p, _f, _i, _i, _i, _i, _i, _i, _p, _p],
+    'pf_window_attention_batched': [_p, _p, _i, _i, _i, _i, _i, _i, _p, _p],
+    'pf_swin_residual_crop_batched': [_p, _p, _i, _i, _i, _i, _i, _i, _p],
     'pf_add_upsampled': [_p, _i, _i, _i, _i, _p, _i, _i, _p, _p],
     'pf_attractor': [_p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],
     'pf_logbinom_depth': [_p, _i, _p, _i, _i, _i, _i, _i, _i, _f, _f, _p, _p],
@@ -83,7 +89,8 @@ SIGNATURES = {
     'pf_stitch_resize': [_p, _p, _i, _i, _i, _i, _p, _p, _p],
 }
 EXPORTS = sorted(list(SIGNATURES) + ['pf_last_error', 'pf_version', 'pf_launch_count', 'pf_branch_workspace_bytes', 'pf_branch_forward',
-                  'pf_g2l_workspace_bytes', 'pf_g2l_forward', 'pf_fusion_workspace_bytes', 'pf_fusion_forward'])
+                  'pf_g2l_workspace_bytes', 'pf_g2l_forward', 'pf_fusion_workspace_bytes', 'pf_fusion_forward',
+                  'pf_fusion_forward_batched'])
 
 _lib = None
 

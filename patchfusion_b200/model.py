@@ -105,7 +105,7 @@ def generatemask(size):
 
 class TiledModel(ParamTree):
     """What `PatchFusion` and `BaselinePretrain` share, as the reference's `PatchFusion(BaselinePretrain)` does: tile
-    configuration, `make_lr`, blend masks, CUDA-graph replay, and the tiled forward of one image (regular passes
+    configuration, `make_lr`, blend masks, CUDA-graph replay, and the tiled forward of a batch of images (regular passes
     flattened into one ordered tile list, the random phase, the deterministic stitch and the tile sharding).  The
     subclass supplies `compute(phase, img, geom, tiles, shard, plan)`: this rank's prediction block of the tile list."""
 
@@ -166,14 +166,16 @@ class TiledModel(ParamTree):
     @torch.no_grad()
     def make_lr(self, image_hr):
         """`image_lr = model.resizer(image)` of `tools/test_single_forward.py:13-14` on the device (same bilinear
-        align_corners=True resample, pf_crop_resize with one whole-image tile)."""
+        align_corners=True resample, pf_crop_resize with one whole-image tile per image): [B,3,H,W] -> [B,3,ph,pw]."""
         from . import ops
-        img = image_hr[0].float().contiguous()
+        img = image_hr.float().contiguous()
+        B = img.shape[0]
         H, W = img.shape[-2:]
         ph, pw = self.resizer.out_size(H, W)
-        out = torch.empty((1, 3, ph, pw), dtype=torch.float32, device=img.device)
-        org = torch.zeros((1, 2), dtype=torch.int32, device=img.device)
-        ops.call('pf_crop_resize', img, H, W, org, 1, H, W, ph, pw, out, ops.stream_ptr())
+        out = torch.empty((B, 3, ph, pw), dtype=torch.float32, device=img.device)
+        org = torch.zeros((B, 2), dtype=torch.int32, device=img.device)
+        index = torch.arange(B, dtype=torch.int32, device=img.device) if B > 1 else None
+        ops.crop_resize(img, org, index, H, W, ph, pw, out)
         return out
 
     def _mask(self, size, device):
@@ -240,31 +242,34 @@ class TiledModel(ParamTree):
         from .parallel import gather_blocks
         return gather_blocks(compute(shard), shard[1], group)
 
-    def _stitch_phase(self, eng, phase, full, origins, world, th, tw, mask, up, base, canvas, want, plan=None):
-        """pf_stitch_gather over the global tile list (deterministic order) -> requested canvases."""
+    def _stitch_phase(self, eng, phase, full, origins, slots, th, tw, mask, up, base, canvas, want, avg_out=None):
+        """pf_stitch_gather of one image's tiles (deterministic order; tile i is row slots[i] of the gathered
+        predictions `full`) -> requested canvases.  avg_out: the [CH, CW] tensor the average is written into."""
         from . import ops
-        from .parallel import slot_table
         CH, CW = canvas
         n = len(origins)
-        slots = slot_table(n, world, plan)
         tab = eng.buf('stitch.tab.' + phase, (n, 3), torch.int32)
         tab.copy_(torch.tensor([(oy, ox, sl) for (oy, ox), sl in zip(origins, slots)], dtype=torch.int32))
         dev = full.device
-        outs = {k: torch.empty((CH, CW), dtype=torch.float32, device=dev) for k in want}
+        outs = {k: torch.empty((CH, CW), dtype=torch.float32, device=dev) for k in want if k != 'avg' or avg_out is None}
+        if 'avg' in want and avg_out is not None:
+            outs['avg'] = avg_out
         ops.call('pf_stitch_gather', full, tab, n, th, tw, mask, up[0], up[1],
                  base[0] if base else None, base[1] if base else None, CH, CW,
                  outs.get('num'), outs.get('den'), outs.get('avg'), ops.stream_ptr())
         return outs
 
-    def _draw_random_boxes(self, n_calls, process_num, H, W, h, w, shard, group, dev):
-        """Random tile origins in the reference's draw order (baseline_pretrain.py:155-156: process_num rows, then ONE
-        shared column per call).  Under real sharding rank 0's draws are broadcast so every rank stitches the same
-        list (all ranks still advance their own `random` state identically)."""
+    def _draw_random_boxes(self, n_calls, process_num, H, W, h, w, shard, group, dev, n_images=1):
+        """Random tiles (image, y, x), image by image, each in the reference's draw order (baseline_pretrain.py:155-156:
+        process_num rows, then ONE shared column per call): the draws of B sequential single-image calls.  Under real
+        sharding rank 0's draws are broadcast once for the batch so every rank stitches the same list (all ranks still
+        advance their own `random` state identically)."""
         boxes = []
-        for _ in range(n_calls):
-            ys = [random.randint(0, H - h - 1) for _ in range(process_num)]
-            x0 = random.randint(0, W - w - 1)
-            boxes += [(y, x0) for y in ys]
+        for b in range(n_images):
+            for _ in range(n_calls):
+                ys = [random.randint(0, H - h - 1) for _ in range(process_num)]
+                x0 = random.randint(0, W - w - 1)
+                boxes += [(b, y, x0) for y in ys]
         if shard is not None and shard[0] != 'emulate' and boxes:
             import torch.distributed as dist
             t = torch.tensor(boxes, dtype=torch.int32, device=dev if dist.get_backend(group) == 'nccl' else 'cpu')
@@ -272,15 +277,41 @@ class TiledModel(ParamTree):
             boxes = [tuple(b) for b in t.cpu().tolist()]
         return boxes
 
+    @staticmethod
+    def batch_tiles(tiles, n_images):
+        """The batch's tile list: every image's tiles (y, x) in their single-image order, image-major, as
+        (image, y, x).  Tile i of image b is item b * len(tiles) + i."""
+        return [(b, y, x) for b in range(n_images) for (y, x) in tiles]
+
+    @staticmethod
+    def image_ranges(items, n_images):
+        """[start, stop) of each image's items in an image-major list of (image, ...) items."""
+        starts = [0] * (n_images + 1)
+        for it in items:
+            starts[it[0] + 1] += 1
+        for b in range(n_images):
+            starts[b + 1] += starts[b]
+        return [(starts[b], starts[b + 1]) for b in range(n_images)]
+
+    @staticmethod
+    def split_tiles(tiles):
+        """Tile list -> ([(y, x)], [image]).  Plain (y, x) tiles belong to image 0 (single-image callers)."""
+        yx = [t[-2:] for t in tiles]
+        return yx, [t[0] if len(t) == 3 else 0 for t in tiles]
+
     def _tiled_forward(self, eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_random_calls, compute,
                        image_lr=None, plan_fn=None):
-        """Tiled inference of one image: the regular passes (baseline_pretrain.py:221-331, patchfusion.py:417-439) are
-        independent tiles whose stitch is a weighted sum, so all passes are flattened into one ordered tile list and
-        micro-batched; rN modes then resize the canvas to image_raw_shape and add `n_random_calls` calls of
-        `process_num` random tiles.  image_lr (PatchFusion) goes into its static buffer; plan_fn(n) gives the rank of
-        each regular tile (None: round-robin)."""
+        """Tiled inference of a batch of B images sharing one tile_cfg: the regular passes
+        (baseline_pretrain.py:221-331, patchfusion.py:417-439) are independent tiles whose stitch is a weighted sum, so
+        all passes of all images are flattened into one ordered, image-major tile list of (image, y, x) and
+        micro-batched (a micro-batch may mix images); rN modes then resize each canvas to image_raw_shape and add
+        `n_random_calls` calls of `process_num` random tiles per image.  The stitch runs once per image over that
+        image's part of the list, so image b's canvas equals its single-image run bit for bit.  image_lr (PatchFusion)
+        goes into its static buffer; plan_fn(n) gives the rank of each regular tile (None: round-robin)."""
         from . import ops
+        from .parallel import slot_table
         dev = image_hr.device
+        B = image_hr.shape[0]
         H, W = tile_cfg['image_raw_shape']
         assert tuple(image_hr.shape[-2:]) == (H, W), 'image_hr must already be at image_raw_shape'
         h, w = tile_cfg['patch_raw_shape']
@@ -289,10 +320,11 @@ class TiledModel(ParamTree):
         geom = (H, W, h, w, ph, pw)
         world = 1 if shard is None else shard[1]
         # inputs into static buffers (stable addresses for the captured graphs)
-        img = eng.buf('in.image_hr', (3, H, W), torch.float32)
-        img.copy_(image_hr[0])
+        img = eng.buf('in.image_hr', (B, 3, H, W), torch.float32)
+        img.copy_(image_hr)
         if image_lr is not None:
-            eng.buf('in.image_lr', (1, 3, ph, pw), torch.float32).copy_(image_lr)
+            assert image_lr.shape[0] == B, 'image_lr and image_hr must hold the same number of images'
+            eng.buf('in.image_lr', (B, 3, ph, pw), torch.float32).copy_(image_lr)
         mask = self._mask((ph, pw), dev)
         offsets = [((0, 0), (0, 0))]
         if cai_mode == 'm2' or cai_mode[0] == 'r':
@@ -304,30 +336,45 @@ class TiledModel(ParamTree):
             raw += [(h * a + oy, w * b + ox) for a in range(ny) for b in range(nx)]
             proc += [(ph * a + py, pw * b + px) for a in range(ny) for b in range(nx)]
         is_r = cai_mode[0] == 'r'
-        plan = plan_fn(len(raw)) if plan_fn is not None else None
-        full = self._exchange(lambda sh: compute('reg', img, geom, raw, sh, plan), shard, group)
-        outs = self._stitch_phase(eng, 'reg', full, proc, world, ph, pw, mask, (0, 0), None, (RH, RW),
-                                  ('num', 'den') if is_r else ('avg',), plan)
-        if is_r:
-            n2 = torch.empty((H, W), dtype=torch.float32, device=dev)
-            d2 = torch.empty_like(n2)
-            ops.call('pf_stitch_resize', outs['num'], outs['den'], RH, RW, H, W, n2, d2, ops.stream_ptr())
-            boxes = self._draw_random_boxes(n_random_calls, process_num, H, W, h, w, shard, group, dev)
-            if boxes:
-                mask_r = self._mask((h, w), dev)
-                base = (n2, d2)
-                chunks = self._chunks(len(boxes), self.random_chunk)
-                for s0, s1 in chunks:
-                    part = boxes[s0:s1]
-                    last = s1 == len(boxes)
-                    full = self._exchange(lambda sh: compute('rnd', img, geom, part, sh, None), shard, group)
-                    outs = self._stitch_phase(eng, 'rnd', full, part, world, ph, pw, mask_r, (h, w), base, (H, W),
-                                              ('avg',) if last else ('num', 'den'))
-                    if not last:
-                        base = (outs['num'], outs['den'])
-            else:
-                outs = {'avg': n2 / d2}
-        return outs['avg'][None, None]
+        tiles = self.batch_tiles(raw, B)
+        plan = plan_fn(len(tiles)) if plan_fn is not None else None
+        full = self._exchange(lambda sh: compute('reg', img, geom, tiles, sh, plan), shard, group)
+        slots = slot_table(len(tiles), world, plan)
+        n = len(raw)
+        CH, CW = (H, W) if is_r else (RH, RW)
+        depth = torch.empty((B, 1, CH, CW), dtype=torch.float32, device=dev)
+        bases = []
+        for b in range(B):
+            outs = self._stitch_phase(eng, 'reg', full, proc, slots[b * n:(b + 1) * n], ph, pw, mask, (0, 0), None,
+                                      (RH, RW), ('num', 'den') if is_r else ('avg',), avg_out=depth[b, 0])
+            if is_r:
+                n2 = torch.empty((H, W), dtype=torch.float32, device=dev)
+                d2 = torch.empty_like(n2)
+                ops.call('pf_stitch_resize', outs['num'], outs['den'], RH, RW, H, W, n2, d2, ops.stream_ptr())
+                bases.append((n2, d2))
+        if not is_r:
+            return depth
+        boxes = self._draw_random_boxes(n_random_calls, process_num, H, W, h, w, shard, group, dev, B)
+        if not boxes:
+            for b, (n2, d2) in enumerate(bases):
+                torch.div(n2, d2, out=depth[b, 0])
+            return depth
+        mask_r = self._mask((h, w), dev)
+        last_of = [r[1] for r in self.image_ranges(boxes, B)]     # end of each image's random tiles
+        for s0, s1 in self._chunks(len(boxes), self.random_chunk):
+            part = boxes[s0:s1]
+            full = self._exchange(lambda sh: compute('rnd', img, geom, part, sh, None), shard, group)
+            slots = slot_table(len(part), world)
+            for b, (i0, i1) in enumerate(self.image_ranges(part, B)):
+                if i0 == i1:
+                    continue
+                last = s0 + i1 == last_of[b]
+                outs = self._stitch_phase(eng, 'rnd', full, [t[1:] for t in part[i0:i1]], slots[i0:i1], ph, pw,
+                                          mask_r, (h, w), bases[b], (H, W), ('avg',) if last else ('num', 'den'),
+                                          avg_out=depth[b, 0])
+                if not last:
+                    bases[b] = (outs['num'], outs['den'])
+        return depth
 
 
 class PatchFusion(TiledModel, PyTorchModelHubMixin):
@@ -352,14 +399,19 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         self.consistency_training = False
         self._runtime_init()
         self._coarse = None
-        # coarse branch + G2L (batch 1) on a side stream next to the first fine branch: measured in DESIGN.md
+        # coarse branch + G2L (batch B) on a side stream next to the first fine branch: measured in DESIGN.md
         self.overlap_coarse = os.environ.get('PF_B200_OVERLAP_COARSE', '1') != '0'
         self._side_stream = None
-        # tile-sharded forward: 'owner' = rank 0 computes the per-image coarse branch + G2L, takes `owner_cost_tiles`
-        # fewer tiles and broadcasts the packed result; 'replicate' = every rank computes it (no broadcast)
+        # tile-sharded forward: 'owner' = rank b % world computes image b's coarse branch + G2L, takes
+        # `owner_cost_tiles` fewer tiles per image it owns, and one all-gather of the packed results reaches every
+        # rank; 'replicate' = every rank computes all of them (no exchange)
         self.shard_coarse = os.environ.get('PF_B200_SHARD_COARSE', 'owner')
         self.owner_cost_tiles = float(os.environ.get('PF_B200_OWNER_COST', '2.7'))
         self._pack = None
+        self._items = None
+        self._local_coarse = {}
+        self._pending_fine = {}
+        self._coarse_src = 'local'
         self._hook_invalidate()
         if config.load_branch:
             for which, path in zip(('coarse_branch', 'fine_branch'), config.pretrain_model):
@@ -392,7 +444,8 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
 
     def invalidate(self):
         super().invalidate()
-        self._pack = None
+        self._pack = self._items = None
+        self._local_coarse = {}
 
     # ------------------------------------------------------------------ stage-level entry points (NCHW fp32 views)
     @staticmethod
@@ -454,77 +507,149 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         return eng.fusion(crops, boxes, fd, ff, cd, cf, g2l)[:, None].clone()
 
     # ------------------------------------------------------------------ tiling
-    def _coarse_stage(self, eng, lr, pack=False):
-        """coarse branch + G2L of the whole image.  pack=True (tile-sharded owner): the results are copied into the
-        contiguous pack buffer that is broadcast, and every later stage reads the pack."""
+    def _coarse_stage(self, eng, lr, pack=None):
+        """coarse branch + G2L of the images `lr` [k,3,ph,pw], at batch k.  pack (tile-sharded owner): this rank's
+        pack views (see _ensure_pack); the results are copied into its first k images, for the all-gather."""
         cd, cf = eng.branch('coarse', lr)
-        res = (cd[0], cf, eng.g2l(cf))
-        if not pack:
-            self._coarse = res
+        res = (cd, cf, eng.g2l(cf))
+        if pack is None:
+            # a replayed graph does not run this method: _compute_phase restores the views of this batch size
+            self._coarse = self._local_coarse[lr.shape[0]] = res
             return
-        dst = self._pack[1]
-        dst[0].copy_(res[0])
-        for d, m in zip(dst[1] + dst[2], res[1] + res[2]):
-            d.t.copy_(m.t)
-        self._coarse = dst
+        k = lr.shape[0]
+        pack[0][:k].copy_(res[0])
+        for d, m in zip(pack[1] + pack[2], res[1] + res[2]):
+            d.t[:k].copy_(m.t)
 
-    def _ensure_pack(self, eng, lr):
-        """Pack buffer for the coarse results (coarse depth fp32, 6 coarse maps, 6 G2L maps; 256-B aligned segments).
-        Its layout follows from the model geometry alone; the first call runs the coarse stage once to read the
-        shapes off the stage outputs (every rank, outside any timed region)."""
-        if self._pack is not None and self._pack[2] is eng:
-            self._coarse = self._pack[1]
-            return self._pack[0]
+    def _coarse_items(self, eng, lr):
+        """(shape of one image, dtype, logical channels or None) of the 13 coarse results: coarse depth fp32, 6 coarse
+        maps, 6 G2L maps.  They follow from the model geometry alone; the first call runs the coarse stage once on one
+        image to read them off the stage outputs (every rank, outside any timed region)."""
+        if getattr(self, '_items', None) is None or self._items[1] is not eng:
+            cd, cf = eng.branch('coarse', lr[:1])
+            g2l = eng.g2l(cf)
+            items = [(tuple(cd.shape[1:]), torch.float32, None)] + \
+                [(tuple(m.t.shape[1:]), m.t.dtype, m.C) for m in cf + g2l]
+            self._items = (items, eng)
+        return self._items[0]
+
+    def _ensure_pack(self, eng, lr, kmax, world):
+        """Buffers of the coarse-owner exchange for ranks that own up to `kmax` images each: this rank's pack (the 13
+        results of kmax images in 256-B aligned segments) and the [world, pack] all-gather destination.  Returns
+        (pack bytes, pack views, gathered bytes, per-rank views into the gathered buffer)."""
+        key = (eng, kmax, world)
+        if self._pack is not None and self._pack[0] == key:
+            return self._pack[1]
         from .engine import Map
-        cd, cf = eng.branch('coarse', lr)
-        g2l = eng.g2l(cf)
-        items = [(cd[0].shape, torch.float32, None)] + [(m.t.shape, m.t.dtype, m.C) for m in cf + g2l]
+        items = self._coarse_items(eng, lr)
         offs, total = [], 0
         for shape, dt, _ in items:
             offs.append(total)
-            total += (int(np.prod(shape)) * torch.empty((), dtype=dt).element_size() + 255) // 256 * 256
-        buf = eng.buf('coarse.pack', (total,), torch.uint8)
-        views = []
-        for (shape, dt, C), o in zip(items, offs):
-            nb = int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
-            t = buf[o:o + nb].view(dt).view(tuple(shape))
-            views.append(t if C is None else Map(t, C))
-        self._pack = (buf, (views[0], views[1:1 + len(cf)], views[1 + len(cf):]), eng)
-        self._coarse = self._pack[1]
-        return buf
+            total += (kmax * int(np.prod(shape)) * torch.empty((), dtype=dt).element_size() + 255) // 256 * 256
 
-    def _fine_stage(self, eng, img, T, geom, raw):
-        """crop+resize -> fine branch for the T tiles whose raw origins are the device rows `raw` ([T,2] int32)."""
+        def views(buf):
+            out = []
+            for (shape, dt, C), o in zip(items, offs):
+                nb = kmax * int(np.prod(shape)) * torch.empty((), dtype=dt).element_size()
+                t = buf[o:o + nb].view(dt).view((kmax,) + tuple(shape))
+                out.append(t if C is None else Map(t, C))
+            return out[0], out[1:7], out[7:]
+        pack = eng.buf('coarse.pack', (total,), torch.uint8)
+        gathered = eng.buf('coarse.gathered', (world, total), torch.uint8)
+        res = (pack, views(pack), gathered, [views(gathered[r]) for r in range(world)])
+        self._pack = (key, res)
+        return res
+
+    def _batch_coarse(self, eng, lr, B):
+        """The batch-B coarse results every fusion of a tile-sharded owner-mode forward reads (the all-gathered packs
+        are copied into them image by image)."""
+        from .engine import Map
+        items = self._coarse_items(eng, lr)
+        out = []
+        for i, (shape, dt, C) in enumerate(items):
+            t = eng.buf('coarse.batch.%d' % i, (B,) + tuple(shape), dt)
+            out.append(t if C is None else Map(t, C))
+        return out[0], out[1:7], out[7:]
+
+    def _exchange_coarse(self, eng, lr, B, rank, world, group, real):
+        """Coarse-owner mode: image b's coarse branch + G2L run on rank b % world, at the batch of that rank's images;
+        every rank packs its results and ONE all-gather of the equal-size packs gives everybody all B images, which
+        are unpacked into the batch-B coarse buffers.  Emulated sharding runs every rank's coarse stage here, at the
+        first rank computed."""
+        from .parallel import coarse_owners, unpack_owned
+        owners = coarse_owners(B, world)
+        kmax = -(-B // world)
+        pack, pviews, gathered, gviews = self._ensure_pack(eng, lr, kmax, world)
+        geom = tuple(lr.shape)
+        for r in (range(world) if not real else [rank]):
+            mine = [b for b in range(B) if owners[b] == r]
+            if not mine:
+                continue
+            lr_r = eng.buf('in.image_lr.owned', (len(mine),) + tuple(lr.shape[1:]), torch.float32)
+
+            def stage(mine=mine, lr_r=lr_r):
+                for j, b in enumerate(mine):
+                    lr_r[j].copy_(lr[b])
+                self._coarse_stage(eng, lr_r, pack=pviews)
+            self._graphed(('coarse.pack', tuple(mine), kmax, B, r, world) + geom, stage)
+            if not real:
+                gathered[r].copy_(pack)
+        if real:
+            self._gather_packs(pack, gathered, group)
+        batch = self._batch_coarse(eng, lr, B)
+        unpack_owned(batch[0], [g[0] for g in gviews], world)
+        for i in range(6):
+            unpack_owned(batch[1][i].t, [g[1][i].t for g in gviews], world)
+            unpack_owned(batch[2][i].t, [g[2][i].t for g in gviews], world)
+        self._coarse = batch
+
+    @staticmethod
+    def _gather_packs(pack, gathered, group):
+        import torch.distributed as dist
+        if dist.get_backend(group) == 'nccl':
+            dist.all_gather_into_tensor(gathered.view(-1), pack, group=group)
+        else:                                   # gloo: list form
+            dist.all_gather(list(gathered.unbind(0)), pack, group=group)
+
+    def _fine_stage(self, eng, img, T, geom, raw, tile_image=None):
+        """crop+resize -> fine branch for the T tiles whose raw origins are the device rows `raw` ([T,2] int32) of the
+        images tile_image ([T] int32, None: image 0) of img ([B,3,H,W] or [3,H,W])."""
         from . import ops
         H, W, h, w, ph, pw = geom
         crops = eng.buf('tile.crops', (T, 3, ph, pw), torch.float32)
-        ops.call('pf_crop_resize', img, H, W, raw, T, h, w, ph, pw, crops, ops.stream_ptr())
+        ops.crop_resize(img, raw, tile_image, h, w, ph, pw, crops)
         # ONE arena for the tile stages, sized for the largest micro-batch: [fine branch | fusion]
         nb = (eng.branch_bytes('fine', T) + 255) // 256 * 256
         arena = eng.arena('tile', nb + eng.fusion_bytes(T, self._coarse[2]))
         fd, ff = eng.branch('fine', crops, ws=(arena, 0))
         return crops, fd, ff, (arena, nb)
 
-    def _fusion_stage(self, eng, fine, boxes, out):
-        """guided fusion of one micro-batch; the fused depth goes straight into its rows `out` of the prediction block."""
+    def _fusion_stage(self, eng, fine, boxes, out, tile_image=None):
+        """guided fusion of one micro-batch; the fused depth goes straight into its rows `out` of the prediction block.
+        tile_image: the image of the batch-B coarse results each tile reads (None: image 0)."""
         cd, cf, g2l = self._coarse
         crops, fd, ff, ws = fine
-        eng.fusion(crops, boxes, fd, ff, cd, cf, g2l, depth_out=out, ws=ws)
+        eng.fusion(crops, boxes, fd, ff, cd, cf, g2l, depth_out=out, ws=ws, tile_image=tile_image)
 
-    def _image_stage(self, eng, lr, img, geom, sizes, io_raw, io_box, blk, with_coarse, part='all'):
-        """The static kernel sequence of one phase of one image on this rank: [coarse branch + G2L] and the
-        micro-batches (fine branch + fusion each).  The coarse stage has no dependency on the first fine branch, so it
-        runs on a side stream next to it (its batch-1 kernels fill a fraction of the SMs).
-        part='pre' / 'post' (tile-sharded, non-owner ranks): the fine branch of the first micro-batch runs BEFORE the
-        broadcast of the owner's coarse results arrives, everything else after it."""
+    def _image_stage(self, eng, lr, img, geom, sizes, io_raw, io_box, io_img, blk, with_coarse, part='all'):
+        """The static kernel sequence of one phase of the batch on this rank: [coarse branch + G2L of the B images]
+        and the micro-batches (fine branch + fusion each; a micro-batch may mix images, io_img gives each tile's).
+        The coarse stage has no dependency on the first fine branch, so it runs on a side stream next to it (its
+        whole-image kernels fill a fraction of the SMs).
+        part='pre' / 'post' (tile-sharded, ranks that own no coarse stage): the fine branch of the first micro-batch
+        runs BEFORE the all-gather of the owners' coarse results arrives, everything else after it."""
         from . import lib
+        ti = (lambda s0, s1: None) if io_img is None else (lambda s0, s1: io_img[s0:s1])
+        # the fine outputs of 'pre' are views whose addresses depend on its micro-batch size only: kept per size, so a
+        # 'post' captured after a replayed 'pre' (which runs no Python) reads the right ones
         if part == 'pre':
-            self._pending_fine = self._fine_stage(eng, img, sizes[0], geom, io_raw[:sizes[0]])
+            self._pending_fine[sizes[0]] = self._fine_stage(eng, img, sizes[0], geom, io_raw[:sizes[0]], ti(0, sizes[0]))
             return
+        s0 = 0
         if part == 'post':
             T0 = sizes[0]
-            self._fusion_stage(eng, self._pending_fine, io_box[:T0], blk[:T0])
-            io_raw, io_box, blk, sizes = io_raw[T0:], io_box[T0:], blk[T0:], sizes[1:]
+            self._fusion_stage(eng, self._pending_fine[T0], io_box[:T0], blk[:T0], ti(0, T0))
+            s0, sizes = T0, sizes[1:]
         cur = torch.cuda.current_stream()
         side = None
         if with_coarse:
@@ -537,88 +662,97 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
                     self._coarse_stage(eng, lr)
             else:
                 self._coarse_stage(eng, lr)
-        s0 = 0
         for T in sizes:
-            fine = self._fine_stage(eng, img, T, geom, io_raw[s0:s0 + T])
+            fine = self._fine_stage(eng, img, T, geom, io_raw[s0:s0 + T], ti(s0, s0 + T))
             if side is not None:
                 cur.wait_stream(side)
                 side = None
-            self._fusion_stage(eng, fine, io_box[s0:s0 + T], blk[s0:s0 + T])
+            self._fusion_stage(eng, fine, io_box[s0:s0 + T], blk[s0:s0 + T], ti(s0, s0 + T))
             s0 += T
 
     def _compute_phase(self, eng, phase, lr, img, geom, raw, process_num, shard, plan=None, group=None):
-        """Fused predictions of this rank's tiles of the (global, ordered) tile list `raw` -> its block
-        [block_rows, ph, pw] fp32 (row j = the j-th tile of the list that `plan` gives to this rank)."""
+        """Fused predictions of this rank's tiles of the (global, ordered) tile list `raw` ((image, y, x) items) ->
+        its block [block_rows, ph, pw] fp32 (row j = the j-th tile of the list that `plan` gives to this rank)."""
         from .parallel import shard_indices, block_rows
         H, W, h, w, ph, pw = geom
         rank, world = (0, 1) if shard is None else shard
+        B = lr.shape[0]
         n = len(raw)
         own = shard_indices(n, rank, world, plan)
         blk = eng.buf('pred.blk.' + phase, (block_rows(n, world, plan), ph, pw), torch.float32)
         with_coarse = phase == 'reg'
         owner_mode = with_coarse and shard is not None and self.shard_coarse == 'owner'
         real = shard is not None and self._real_shard
+        owns_coarse = owner_mode and rank < B               # image b's coarse stage runs on rank b % world
+        split = owner_mode and real and not owns_coarse and bool(own)
+        if with_coarse and not owner_mode:
+            # the views the coarse stage of this batch size last produced: valid whenever its graph is (both are
+            # renewed when a workspace moves), and what the later 'rnd' phase of this forward reads
+            self._coarse = self._local_coarse.get(B, self._coarse)
         if owner_mode:
-            # rank 0 computes coarse + G2L into the pack and broadcasts it; the others start on their fine branch
-            pack = self._ensure_pack(eng, lr)
-            if rank == 0:
-                self._graphed(('coarse.pack',) + tuple(geom), lambda: self._coarse_stage(eng, lr, pack=True))
             with_coarse = False
+            if split:
+                self._coarse = self._batch_coarse(eng, lr, B)   # shapes for the 'pre' stage; filled by the exchange
+            elif real or rank == 0:                             # emulated ranks run in order: rank 0 does them all
+                self._exchange_coarse(eng, lr, B, rank, world, group, real)
         if not own:
-            if owner_mode and real:
-                self._broadcast_pack(pack, group)
             return blk
         io_raw = eng.buf('io.raw.' + phase, (len(own), 2), torch.int32)
         io_box = eng.buf('io.box.' + phase, (len(own), 4), torch.float32)
         fx, fy = np.float32(1 / W * pw), np.float32(1 / H * ph)
-        chunk = [raw[i] for i in own]
+        chunk, images = self.split_tiles([raw[i] for i in own])
         io_raw.copy_(torch.tensor(chunk, dtype=torch.int32))
+        io_img = None
+        if B > 1:
+            io_img = eng.buf('io.img.' + phase, (len(own),), torch.int32)
+            io_img.copy_(torch.tensor(images, dtype=torch.int32))
         # boxes exactly as baseline_pretrain.py:268-282: int pixel box * fp32 factor
         io_box.copy_(torch.from_numpy(np.array(
             [[np.float32(x) * fx, np.float32(y) * fy, np.float32(x + w) * fx, np.float32(y + h) * fy]
              for (y, x) in chunk], dtype=np.float32)))
         sizes = self._micro_sizes(len(own), process_num)
-        key = ('image', phase, tuple(sizes), blk.shape[0], with_coarse) + tuple(geom)
+        key = ('image', phase, tuple(sizes), blk.shape[0], with_coarse, B, self._coarse_src) + tuple(geom)
         run = lambda part: self._graphed(key + (part,), lambda: self._image_stage(
-            eng, lr, img, geom, sizes, io_raw, io_box, blk, with_coarse, part))
-        if owner_mode and real:
-            if rank != 0:
-                run('pre')
-            self._broadcast_pack(pack, group)
-            run('post' if rank != 0 else 'all')
+            eng, lr, img, geom, sizes, io_raw, io_box, io_img, blk, with_coarse, part))
+        if split:
+            run('pre')
+            self._exchange_coarse(eng, lr, B, rank, world, group, real)
+            run('post')
         else:
             run('all')
         return blk
 
-    @staticmethod
-    def _broadcast_pack(pack, group):
-        import torch.distributed as dist
-        dist.broadcast(pack, src=dist.get_global_rank(group, 0) if group is not None else 0, group=group)
-
     @torch.no_grad()
     def forward(self, mode, image_lr, image_hr, depth_gt=None, crops_image_hr=None, crop_depths=None, bboxs=None,
                 tile_cfg=None, cai_mode='m1', process_num=4, shard=None, group=None):
-        """`shard=(rank, world)` (extension): this rank runs tiles rank, rank+world, ... of the flattened tile list and
-        ONE all-gather of the per-rank prediction blocks (patchfusion_b200/parallel.py) precedes the deterministic
-        stitch, so the canvas is bit-identical to the single-device one.  `group`: the process group of `world` ranks
-        (default group if None).  shard=None reproduces the reference's single-device behaviour."""
+        """image_lr [B,3,ph,pw], image_hr [B,3,H,W] -> depth [B,1,H',W'] (extension: the reference takes B = 1).  All B
+        images share tile_cfg, cai_mode and process_num; their tiles form one image-major list that is micro-batched
+        and sharded together, the coarse branch + G2L run once at batch B, and image b's output equals, bit for bit,
+        the single-image call on it made after images 0..b-1 from the same `random` state.
+        `shard=(rank, world)` (extension): this rank runs its share of the flattened tile list and ONE all-gather of
+        the per-rank prediction blocks (patchfusion_b200/parallel.py) precedes the deterministic stitch, so the canvas
+        is bit-identical to the single-device one.  `group`: the process group of `world` ranks (default group if
+        None).  shard=None reproduces the reference's single-device behaviour."""
         if mode == 'train':
             raise NotImplementedError('training is out of scope of the H100 hot-path build (SURVEY.md §2 rows 10,12)')
         if tile_cfg is None:
             tile_cfg = self.tile_cfg
         else:
             tile_cfg = self.prepare_tile_cfg(tile_cfg['image_raw_shape'], tile_cfg['patch_split_num'])
-        assert image_hr.shape[0] == 1
+        B = image_hr.shape[0]
+        assert B >= 1 and image_lr.shape[0] == B, 'image_lr and image_hr must hold the same number (>= 1) of images'
         self._check_shard(shard, group)
         eng = self.engine()
         ph, pw = self.patch_process_shape
         plan_fn = None
-        if shard is not None and self.shard_coarse == 'owner':
+        owner = shard is not None and self.shard_coarse == 'owner'
+        self._coarse_src = 'gathered' if owner else 'local'
+        if owner:
             from .parallel import tile_plan
-            plan_fn = lambda n: tile_plan(n, shard[1], self.owner_cost_tiles)
+            plan_fn = lambda n: tile_plan(n, shard[1], self.owner_cost_tiles, images=B)
 
         def compute(phase, img, geom, tiles, sh, plan):
-            lr = eng.buf('in.image_lr', (1, 3, ph, pw), torch.float32)
+            lr = eng.buf('in.image_lr', (B, 3, ph, pw), torch.float32)
             return self._compute_phase(eng, phase, lr, img, geom, tiles, process_num, sh, plan, group)
 
         # patchfusion.py:441-448: N // process_num calls of process_num random tiles

@@ -164,16 +164,25 @@ def resize_bilinear(x, C_, OH, OW, out, out_col0=0):
     call('pf_resize_bilinear', x, B, H, W, pad_to(C_, 8), ld, OH, OW, out, out.shape[-1], out_col0, stream_ptr())
 
 
-def roi_crop_zoom(feat, C_, boxes, scale, out, out_col0=0):
-    """feat [1,h,w,ld] bf16 or [h,w] fp32 (depth); boxes [T,4] fp32 device."""
+def roi_crop_zoom(feat, C_, boxes, scale, out, out_col0=0, tile_image=None):
+    """feat [B,h,w,ld] bf16 or [B,h,w] / [h,w] fp32 (depth); boxes [T,4] fp32 device; tile_image: int32 [T] device
+    tensor, the image of `feat` each box reads (None: image 0)."""
     T = boxes.shape[0]
     if feat.dtype == torch.float32:
         h, w = feat.shape[-2:]
-        call('pf_roi_crop_zoom', feat, 1, h, w, 1, 1, boxes, T, C.c_float(scale), out, 1, 0, stream_ptr())
+        call('pf_roi_crop_zoom_batched', feat, 1, h, w, 1, 1, tile_image, boxes, T, C.c_float(scale), out, 1, 0,
+             stream_ptr())
     else:
         _, h, w, ld = feat.shape
-        call('pf_roi_crop_zoom', feat, 0, h, w, pad_to(C_, 8), ld, boxes, T, C.c_float(scale), out, out.shape[-1],
-             out_col0, stream_ptr())
+        call('pf_roi_crop_zoom_batched', feat, 0, h, w, pad_to(C_, 8), ld, tile_image, boxes, T, C.c_float(scale), out,
+             out.shape[-1], out_col0, stream_ptr())
+
+
+def crop_resize(img, origins, tile_image, th, tw, ph, pw, out):
+    """Tiles of img [B,3,H,W] (or [3,H,W]) fp32: tile t = image tile_image[t] (None: image 0) at origins[t] (int32
+    [T,2] device, y, x), th x tw pixels, resized to out [T,3,ph,pw] (bilinear, align_corners=True)."""
+    H, W = img.shape[-2:]
+    call('pf_crop_resize_batched', img, H, W, origins, tile_image, origins.shape[0], th, tw, ph, pw, out, stream_ptr())
 
 
 def maxpool2(x, C_, out):

@@ -5,25 +5,44 @@ sharded.  Tiles are independent given the per-image coarse outputs and the stitc
 decompositions are offered:
 
 * images-per-rank (bench.py `value`, weak scaling): every rank runs whole images; no data-path collective.
-* tiles-per-rank (`PatchFusion.forward(..., shard=(rank, world))`, SURVEY.md §8e): the per-image coarse branch + G2L
-  (batch-1 kernels, ~2.7 tiles' worth of time) run on rank 0 only, which takes correspondingly fewer tiles
-  (`tile_plan`) and broadcasts the coarse depth, the six coarse maps and the six G2L maps (one packed buffer) while the
-  other ranks are already in the fine branch of their first micro-batch (the fine branch does not read coarse data).
-  Each rank writes its fused predictions into a block [block_rows, ph, pw] and ONE all-gather of those blocks
-  (5.7 MB per rank for 4K P49) lets every rank run the deterministic stitch (pf_stitch_gather) over the global tile
-  list: the canvas is bit-identical to the single-device one for any world size and any plan.
-  `model.shard_coarse = 'replicate'` keeps the collective-free variant (every rank computes the coarse stage).
+* tiles-per-rank (`PatchFusion.forward(..., shard=(rank, world))`, SURVEY.md §8e): the coarse branch + G2L of image b
+  (whole-image kernels, ~2.7 tiles' worth of time) run on rank b % world only (`coarse_owners`), which takes
+  correspondingly fewer tiles (`tile_plan`); every rank packs the coarse depth, six coarse maps and six G2L maps of
+  its images into one buffer and ONE all-gather of those equal-size packs reaches every rank, while the ranks that
+  own no image are already in the fine branch of their first micro-batch (the fine branch does not read coarse data).
+  The tiles of all B images of a batch form one image-major list (tile i of image b is item b * n + i).  Each rank
+  writes its fused predictions into a block [block_rows, ph, pw] and ONE all-gather of those blocks (5.7 MB per rank
+  for one 4K P49 image) lets every rank run the deterministic stitch (pf_stitch_gather) of each image over that
+  image's part of the global slot table: each canvas is bit-identical to the single-device one for any world size and
+  any plan.  `model.shard_coarse = 'replicate'` keeps the variant without the pack exchange (every rank computes the
+  coarse stage of every image).
 """
 import torch
 
 
-def tile_plan(n_items, world, owner_cost=0.0, owner=0):
+def coarse_owners(n_images, world, owner=0):
+    """Rank that computes (and packs for everybody) the coarse branch + G2L of each image of a batch: image b on rank
+    (owner + b) % world."""
+    return [(owner + b) % world for b in range(n_images)]
+
+
+def unpack_owned(dst, packed, world):
+    """dst [B, ...] <- the all-gathered packs: packed[r] ([kmax, ...], a tensor row or list entry per rank) holds rank
+    r's images r, r + world, ... (coarse_owners with owner 0) in its first rows.  One strided copy per rank."""
+    B = dst.shape[0]
+    for r in range(min(world, B)):
+        dst[r::world].copy_(packed[r][:len(range(r, B, world))])
+
+
+def tile_plan(n_items, world, owner_cost=0.0, owner=0, images=1):
     """Rank of every item of the ordered tile list.  Items are handed out one at a time to the least-loaded rank (ties:
-    lowest rank); `owner` starts with `owner_cost` items' worth of work - the per-image coarse branch + G2L it computes
-    and broadcasts for everybody.  owner_cost = 0 is plain round-robin (item i -> rank i % world).  A pure function of
-    its arguments: every rank derives the same plan without communication."""
+    lowest rank); every coarse owner (`coarse_owners(images, world, owner)`) starts with `owner_cost` items' worth of
+    work per image it owns - the coarse branch + G2L it computes and packs for everybody.  owner_cost = 0 is plain
+    round-robin (item i -> rank i % world); images = 1 is the single-image plan (`owner` alone is charged).  A pure
+    function of its arguments: every rank derives the same plan without communication."""
     load = [0.0] * world
-    load[owner] = float(owner_cost)
+    for r in coarse_owners(images, world, owner):
+        load[r] += float(owner_cost)
     plan = []
     for _ in range(n_items):
         r = min(range(world), key=lambda q: (load[q], q))

@@ -84,12 +84,15 @@ def _bind():
     h.pf_fusion_forward.restype = C.c_int
     h.pf_fusion_forward.argtypes = [C.POINTER(PfFusion), vp, vp, i32, vp, C.POINTER(PfMap), vp, C.POINTER(PfMap),
                                     C.POINTER(PfMap), vp, C.c_size_t, vp, vp, vp, vp]
+    h.pf_fusion_forward_batched.restype = C.c_int
+    h.pf_fusion_forward_batched.argtypes = [C.POINTER(PfFusion), vp, vp, vp, i32, vp, C.POINTER(PfMap), vp,
+                                            C.POINTER(PfMap), C.POINTER(PfMap), vp, C.c_size_t, vp, vp, vp, vp]
     _bound = True
     return h
 
 
 STAGE_EXPORTS = ['pf_branch_workspace_bytes', 'pf_branch_forward', 'pf_g2l_workspace_bytes', 'pf_g2l_forward',
-                 'pf_fusion_workspace_bytes', 'pf_fusion_forward']
+                 'pf_fusion_workspace_bytes', 'pf_fusion_forward', 'pf_fusion_forward_batched']
 
 
 def _check(rc, what):
@@ -148,9 +151,12 @@ def g2l_forward(cf, maps, ws_ptr, ws_bytes):
 
 
 def fusion_forward(cf, crops, boxes, T, fine_depth, fine_maps, coarse_depth, coarse_maps, g2l_maps, ws_ptr, ws_bytes,
-                   depth_out, tap=None):
+                   depth_out, tap=None, tile_image=None):
+    """tile_image (int32 [T] device tensor or None): the image of the batch-B coarse inputs each tile reads."""
     cbk = TAP_FN(tap) if tap is not None else None
-    rc = _bind().pf_fusion_forward(C.byref(cf), crops.data_ptr(), boxes.data_ptr(), T, fine_depth.data_ptr(), fine_maps,
-                                   coarse_depth.data_ptr(), coarse_maps, g2l_maps, ws_ptr, ws_bytes, depth_out.data_ptr(),
-                                   C.cast(cbk, vp) if cbk is not None else None, None, lib.stream_ptr())
+    ti = tile_image.data_ptr() if tile_image is not None else None
+    rc = _bind().pf_fusion_forward_batched(C.byref(cf), crops.data_ptr(), boxes.data_ptr(), ti, T, fine_depth.data_ptr(),
+                                           fine_maps, coarse_depth.data_ptr(), coarse_maps, g2l_maps, ws_ptr, ws_bytes,
+                                           depth_out.data_ptr(), C.cast(cbk, vp) if cbk is not None else None, None,
+                                           lib.stream_ptr())
     _check(rc, 'pf_fusion_forward')

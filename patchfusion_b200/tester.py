@@ -35,10 +35,25 @@ class Tester:
             cv2.imwrite(os.path.join(self.work_dir, '%s_uint16.png' % name), raw.numpy())
             q.task_done()
 
+    @staticmethod
+    def _groups(samples, batch_size):
+        """consecutive samples in lists of batch_size (the last one may be shorter), in input order"""
+        group = []
+        for s in samples:
+            group.append(s)
+            if len(group) == batch_size:
+                yield group
+                group = []
+        if group:
+            yield group
+
     @torch.no_grad()
-    def run(self, samples, cai_mode='m1', process_num=4, image_raw_shape=(2160, 3840), patch_split_num=(4, 4)):
+    def run(self, samples, cai_mode='m1', process_num=4, image_raw_shape=(2160, 3840), patch_split_num=(4, 4),
+            batch_size=1):
         """samples: iterable of dicts {'img_file_basename': str, 'image_u8': HxWx3 uint8 BGR (cv2.imread) OR
         'image_hr': (1,3,H,W) fp32 in [0,1], optional 'depth_gt' (1,1,h,w), optional 'boundary'}.
+        batch_size > 1: consecutive samples go through the model together (one batched forward); outputs, files and
+        metrics are those of batch_size 1, in input order.
         Returns the list of per-image metric dicts (empty when no ground truth is given)."""
         model = self.model
         dev = next(model.parameters()).device
@@ -50,40 +65,51 @@ class Tester:
             q = queue.Queue(maxsize=2)
             th = threading.Thread(target=self._writer, args=(q,), daemon=True)
             th.start()
-        for i, s in enumerate(samples):
-            if 'image_hr' in s:
-                image = s['image_hr'].to(dev, non_blocking=True).float()
-            else:
-                image = imageio.ingest(s['image_u8'], tuple(image_raw_shape), dev, bgr=True)
+        i = 0
+        for group in self._groups(samples, max(1, int(batch_size))):
+            images = []
+            for s in group:
+                if 'image_hr' in s:
+                    images.append(s['image_hr'].to(dev, non_blocking=True).float())
+                else:
+                    images.append(imageio.ingest(s['image_u8'], tuple(image_raw_shape), dev, bgr=True))
+            image = images[0] if len(images) == 1 else torch.cat(images)
             lr = model.make_lr(image)
-            result, _ = model(mode='infer', cai_mode=cai_mode, process_num=process_num, tile_cfg=tile_cfg,
-                              image_lr=lr, image_hr=image)
-            if self.save:
-                color = imageio.colorize(result, cmap='gray_r' if self.gray_scale else 'magma_r', bgr=True)
-                raw = imageio.depth_to_u16(result)              # tester.py:75: (result * 256).astype('uint16')
-                k = i % 2
-                if slots[k] is None or slots[k][0].shape != color.shape:
-                    slots[k] = (torch.empty(color.shape, dtype=torch.uint8).pin_memory(),
-                                torch.empty(raw.shape, dtype=torch.uint16).pin_memory())
-                q.join() if i >= 2 and q.unfinished_tasks >= 2 else None
-                ev = torch.cuda.Event()
-                copy_stream.wait_stream(torch.cuda.current_stream(dev))
-                with torch.cuda.stream(copy_stream):
-                    slots[k][0].copy_(color, non_blocking=True)
-                    slots[k][1].copy_(raw, non_blocking=True)
-                    ev.record(copy_stream)
-                color.record_stream(copy_stream)
-                raw.record_stream(copy_stream)
-                q.put((ev, s['img_file_basename'], slots[k][0], slots[k][1]))
-            if s.get('depth_gt') is not None:
-                results.append(pf_metrics.compute_metrics(
-                    s['depth_gt'].to(dev), result, disp_gt_edges=s.get('boundary'), min_depth_eval=self.min_depth,
-                    max_depth_eval=self.max_depth))
+            results_b, _ = model(mode='infer', cai_mode=cai_mode, process_num=process_num, tile_cfg=tile_cfg,
+                                 image_lr=lr, image_hr=image)
+            for j, s in enumerate(group):
+                result = results_b[j:j + 1]
+                self._emit(s, i, result, slots, q, copy_stream, dev, results)
+                i += 1
         if self.save:
             q.join()
             q.put(None)
             th.join()
         return results
+
+    def _emit(self, s, i, result, slots, q, copy_stream, dev, results):
+        """Outputs of sample number i: colour and uint16 PNGs through the writer thread, metrics."""
+        if self.save:
+            color = imageio.colorize(result, cmap='gray_r' if self.gray_scale else 'magma_r', bgr=True)
+            raw = imageio.depth_to_u16(result)              # tester.py:75: (result * 256).astype('uint16')
+            k = i % 2
+            if slots[k] is None or slots[k][0].shape != color.shape:
+                slots[k] = (torch.empty(color.shape, dtype=torch.uint8).pin_memory(),
+                            torch.empty(raw.shape, dtype=torch.uint16).pin_memory())
+            q.join() if i >= 2 and q.unfinished_tasks >= 2 else None
+            ev = torch.cuda.Event()
+            copy_stream.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(copy_stream):
+                slots[k][0].copy_(color, non_blocking=True)
+                slots[k][1].copy_(raw, non_blocking=True)
+                ev.record(copy_stream)
+            color.record_stream(copy_stream)
+            raw.record_stream(copy_stream)
+            q.put((ev, s['img_file_basename'], slots[k][0], slots[k][1]))
+        if s.get('depth_gt') is not None:
+            results.append(pf_metrics.compute_metrics(
+                s['depth_gt'].to(dev), result, disp_gt_edges=s.get('boundary'), min_depth_eval=self.min_depth,
+                max_depth_eval=self.max_depth))
 
     @staticmethod
     def evaluate(results):
