@@ -58,6 +58,13 @@ int pf_set_option(int32_t option, int32_t value);
 int pf_profile_start(void* stream);
 int pf_profile_stop(void);
 int pf_profile_get(int32_t i, const char** name, const char** label, double* flops, float* ms);
+/* pf_gemm_kernel phase timeline, in libraries built with -DPF_GEMM_TIMELINE (any other build returns an error):
+ * synchronises the device, copies the PF_GEMM_TIMELINE_SLOTS clock64 sums accumulated by every pf_gemm_kernel launch
+ * since the last reset into host array `out` (may be NULL) and zeroes them if `reset`.  Slots: producer tiles, producer
+ * cycles waiting for an empty stage, producer loop cycles; then per consumer warpgroup: tiles, cycles waiting for a
+ * full stage, mainloop cycles (waits included), epilogue cycles, loop cycles. */
+#define PF_GEMM_TIMELINE_SLOTS 8
+int pf_gemm_timeline(unsigned long long* out, int32_t reset);
 
 /* ---- dense contractions: one wgmma/TMA implicit-GEMM kernel ----------------------------------------------------
  * Replaces every nn.Linear / nn.Conv2d(1x1, 3x3 s1 p1) / nn.ConvTranspose2d(k==s) on the path:

@@ -152,10 +152,14 @@ __device__ __forceinline__ void ld_shared_v4(uint32_t addr, uint32_t& a, uint32_
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(a), "=r"(b), "=r"(c), "=r"(d) : "r"(addr) : "memory");
 }
 // arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster (release at cluster scope)
+// Arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster.  Default (.release.cta)
+// semantics: the callers release an operand stage whose only readers were wgmma instructions already retired by
+// wgmma.wait_group, so there is nothing left for a cluster-scope release to order.  `.release.cluster` compiles to a
+// MEMBAR.ALL.GPU before every arrive: a GPU-wide fence the releasing warp waited out once per stage and peer CTA.
 __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
 // ---------------------------------------------------------------- ldmatrix

@@ -617,7 +617,32 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
   }
 }
 
-
+// ------------------------------------------------------------------------------------------------------------
+// Phase timeline of pf_gemm_kernel (built only with -DPF_GEMM_TIMELINE; pf_gemm_timeline reads it).  One lane per
+// role records clock64 intervals in registers and adds them to g_gemm_timeline when its CTA retires: the producer
+// (slots 0-2: tiles, cycles waiting for an empty stage, cycles in its loop) and lane 0 of each consumer warpgroup's
+// first warp (slots 3-7: tiles, cycles waiting for a full stage, mainloop cycles including those waits, epilogue
+// cycles, cycles in its loop).  Every other build compiles the stamps to nothing.
+#ifdef PF_GEMM_TIMELINE
+constexpr int kTimelineSlots = 8;
+__device__ unsigned long long g_gemm_timeline[kTimelineSlots];
+struct GemmTimeline {
+  long long v[5] = {0, 0, 0, 0, 0};
+  __device__ __forceinline__ long long now() const { return clock64(); }
+  __device__ __forceinline__ void add(int i, long long t0) { v[i] += clock64() - t0; }
+  __device__ __forceinline__ void tile() { v[0] += 1; }
+  __device__ __forceinline__ void flush(int slot0, int n) const {
+    for (int i = 0; i < n; ++i) atomicAdd(&g_gemm_timeline[slot0 + i], static_cast<unsigned long long>(v[i]));
+  }
+};
+#else
+struct GemmTimeline {
+  __device__ __forceinline__ long long now() const { return 0; }
+  __device__ __forceinline__ void add(int, long long) {}
+  __device__ __forceinline__ void tile() {}
+  __device__ __forceinline__ void flush(int, int) const {}
+};
+#endif
 
 // MC = true: launched as clusters of 2 CTAs that take two m-tiles of the SAME n-tile; each CTA fetches half of the
 // weight tile and multicasts it into both CTAs' shared memory (halves the weight traffic of the linear layers).
@@ -656,16 +681,21 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
     if (warp == kTmaWarp) {
       // ===================== TMA producer =====================
       // whole warp in uniform control flow (coordinates and stage counters in uniform registers), one elected lane issues
+      GemmTimeline tl;
+      const long long tl_start = tl.now();
       int stage = 0; uint32_t phase = 0;
       for (int ti = it.first; ti < it.count; ti += it.step) {
         TileCoord c = decode_tile(d, it.tile(ti));
+        tl.tile();
         int kb = 0;  // running 64-wide K block index into the packed weights
         for (int s = 0; s < d.num_src; ++s) {
           for (int tap = 0; tap < d.taps; ++tap) {
             int dy = d.taps == 9 ? tap / 3 - 1 : 0;
             int dx = d.taps == 9 ? tap % 3 - 1 : 0;
             for (int ch = 0; ch < d.chunks[s]; ++ch, ++kb) {
+              const long long tl_w = tl.now();
               mbar_wait(&empty_bar[stage], phase ^ 1);
+              tl.add(1, tl_w);
               uint8_t* sa = smem + stage * stage_bytes;
               uint8_t* sb = sa + kATileBytes;
               if (elect_one()) {
@@ -685,6 +715,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
           }
         }
       }
+      tl.add(2, tl_start);
+      if (lane == 0) tl.flush(0, 3);
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma mainloop + epilogue =====================
@@ -695,11 +727,17 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
     float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
     int rs = 0;                                             // oldest stage not yet released
+    GemmTimeline tl;
+    const long long tl_start = tl.now();
     for (int ti = it.first; ti < it.count; ti += it.step) {
       const TileCoord c = decode_tile(d, it.tile(ti));
+      tl.tile();
+      const long long tl_main = tl.now();
       uint32_t accum = 0;
       for (int kb = 0; kb < P.k_steps; ++kb) {
+        const long long tl_w = tl.now();
         mbar_wait(&full_bar[stage], phase);
+        tl.add(1, tl_w);
         const uint32_t sa = smem_u32(smem + stage * stage_bytes);
         const uint64_t adesc = wgmma_desc_k128(sa + a_off);
         const uint64_t bdesc = wgmma_desc_k128(sa + kATileBytes);
@@ -718,10 +756,15 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
       wgmma_wait<0>();                                      // the tile's last block is done: its stage is free
       release_stage<CL>(&empty_bar[rs], lane);
       if (++rs == stages) rs = 0;
+      tl.add(2, tl_main);
+      const long long tl_epi = tl.now();
       epilogue_tile(d, c, acc, warp, lane, buf, &et);
       __syncwarp();
+      tl.add(3, tl_epi);
     }
     if (lane == 0) bulk_wait0();    // the staging tiles are read (and the writes performed) before the CTA retires
+    tl.add(4, tl_start);
+    if (lane == 0 && (warp & 3) == 0) tl.flush(3, 5);
   }
   __syncthreads();
   if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
@@ -1128,3 +1171,21 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
 
 
 }  // namespace pf
+
+extern "C" int pf_gemm_timeline(unsigned long long* out, int32_t reset) {
+#ifdef PF_GEMM_TIMELINE
+  static_assert(pf::kTimelineSlots == PF_GEMM_TIMELINE_SLOTS, "timeline slots");
+  cudaError_t e = cudaDeviceSynchronize();
+  if (e == cudaSuccess && out != nullptr)
+    e = cudaMemcpyFromSymbol(out, pf::g_gemm_timeline, sizeof(unsigned long long) * pf::kTimelineSlots);
+  if (e == cudaSuccess && reset) {
+    const unsigned long long zero[pf::kTimelineSlots] = {};
+    e = cudaMemcpyToSymbol(pf::g_gemm_timeline, zero, sizeof(zero));
+  }
+  if (e != cudaSuccess) return pf::set_error("pf_gemm_timeline: %s", cudaGetErrorString(e));
+  return 0;
+#else
+  (void)out; (void)reset;
+  return pf::set_error("pf_gemm_timeline: library built without -DPF_GEMM_TIMELINE");
+#endif
+}

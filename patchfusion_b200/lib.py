@@ -49,6 +49,7 @@ SIGNATURES = {
     'pf_profile_start': [_p],
     'pf_profile_stop': [],
     'pf_profile_get': [_i, _p, _p, _p, _p],
+    'pf_gemm_timeline': [_p, _i],
     'pf_gemm': [C.POINTER(GemmDesc), _p],
     'pf_pack_weight': [_p, _i, _i, _i, C.POINTER(C.c_int32), _i, _p, _p, _p],
     'pf_pack_weight_convT': [_p, _i, _i, _i, _p, _p],
