@@ -19,11 +19,13 @@
 // against all BN columns of the n-tile, one wgmma.m64nBNk16 per k16 step with both operands read by the tensor core
 // from the swizzled TMA tiles in shared memory (every A tile is 128 rows x 128 B in the canonical K-major layout, so
 // the warpgroup's A operand is a descriptor at its 8 KB row offset).  Warp w owns tile rows 16w .. 16w + 15, so after
-// the mainloop every accumulator row lives in one warp.  The same warps then run the epilogue: a 16 x 32 fp32 block at
-// a time goes through a per-warp swizzled shared-memory transpose so that a thread holds 16 columns of one accumulator
-// row (bias / activation / residuals / fused tail per row), then a swizzled staging tile + bulk tensor store (bf16), a
-// bulk reduce-add (the fp32 residual stream), or direct stores for the fused-tail / residual / pixel-shuffle / V^T
-// variants.  The last warp is the TMA producer; the halo kernel has two more warps before it, the operand producers of
+// the mainloop every accumulator row lives in one warp.  The same warps then run the epilogue.  Plain outputs (bias /
+// activation / gamma) are finished in the accumulator's fragment layout, staged 16 rows x 128 B at a time in one of the
+// warp's two swizzled staging tiles (stmatrix for bf16, 8-byte stores for fp32) and moved by a bulk tensor store, or a
+// bulk reduce-add for the fp32 residual stream.  The variants that need a whole row per thread (residuals / fused tail /
+// ReLU copy / pixel shuffle / the V^T third of a fused qkv projection) send a 16 x 32 fp32 block at a time through a per-warp
+// swizzled shared-memory transpose so that a thread holds 16 columns of one accumulator row, and store directly.
+// The last warp is the TMA producer; the halo kernel has two more warps before it, the operand producers of
 // its optional fused bilinear resample (idle otherwise).  While the consumers drain a tile, the producer already fills
 // the operand ring for the next one.
 //
@@ -47,17 +49,19 @@ constexpr int kGemmThreads = (kEpiWarps + 1) * 32;
 constexpr int kHaloThreads = (kEpiWarps + 3) * 32;
 constexpr int kRsWarp0 = kEpiWarps;                         // halo kernel: warps 8, 9 = resample producers
 constexpr int kMaxSmem = 227 * 1024;
-// per consumer warp: the 16 x 32 fp32 accumulator transpose; in pf_gemm_kernel also the staging tile (16 rows x 128 B,
-// SWIZZLE_128B) of the TMA-store epilogue
+// per consumer warp: the 16 x 32 fp32 accumulator transpose of the row-per-thread epilogue.  pf_gemm_kernel has two such
+// blocks per warp, the staging tiles of the TMA-store epilogue (16 rows x 128 B, SWIZZLE_128B) used in turn; the first
+// doubles as the transpose block
 constexpr int kXposeWarp = 16 * 32 * 4;
+constexpr int kStageWarp = 2 * kXposeWarp;
 constexpr int kBarBytes = 512;
 
 // pf_gemm_kernel operand ring: one stage = the 128-row A tile + BN weight rows of one 64-wide K block; as many stages
 // as fit next to the transposes and barriers, at most eight
 __host__ __device__ constexpr int gemm_stage_bytes(int bn) { return kATileBytes + bn * kBlockK * 2; }
 __host__ __device__ constexpr int gemm_stages(int bn) {
-  return (kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kXposeWarp) / gemm_stage_bytes(bn) < 8
-             ? (kMaxSmem - 1024 - kBarBytes - kEpiWarps * kXposeWarp) / gemm_stage_bytes(bn)
+  return (kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kStageWarp) / gemm_stage_bytes(bn) < 8
+             ? (kMaxSmem - 1024 - kBarBytes - kEpiWarps * kStageWarp) / gemm_stage_bytes(bn)
              : 8;
 }
 
@@ -356,28 +360,39 @@ __device__ __forceinline__ void epilogue_row(const GemmDesc& d, const float (&ac
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Epilogue through shared memory + TMA (pf_gemm_kernel, d.tma_out != 0).
-// A thread owns one accumulator row, so direct global accesses are 32-byte pieces of 32 different rows per instruction:
-// one L2 request per sector.  Here each warp stages its 16 rows in a swizzled 2 KB tile and ONE elected lane moves it
-// with a bulk tensor copy: 128-byte requests, no LSU work; the fp32 residual stream is updated by a bulk reduce-add (no
-// read at all).  The staging tile doubles as the warp's transpose block, so the previous copy must have finished
-// reading it before the next accumulator block is staged.
+// Epilogue through shared memory + TMA (pf_gemm_kernel, d.tma_out != 0), in the accumulator's own layout.
+// Bias, activation and the gamma scale are per-column vectors and per-element functions, so they are applied where the
+// accumulator already is: a thread's fragment holds columns 8j + 2 (lane % 4) + {0, 1} of rows lane / 4 and lane / 4 + 8,
+// and adds the bias as one float2 per j.  The warp's 16 rows then go into a swizzled 2 KB staging tile (stmatrix for
+// bf16, 8-byte stores for fp32) and ONE elected lane moves the tile with a bulk tensor copy: 128-byte requests, no LSU
+// work; the fp32 residual stream is updated by a bulk reduce-add (no read at all).  Each warp has two staging tiles
+// and uses them in turn, so a copy reads one while the next block is computed into the other.
 
 struct EpiTma {
   const CUtensorMap* tm;
-  uint32_t stg;        // shared address of this warp's staging tile (1024-B aligned)
+  uint32_t stg;        // shared address of this warp's two staging tiles (1024-B aligned, kXposeWarp bytes each)
   uint8_t* stg_ptr;
+  int cur;             // the tile the next block is staged in
 };
 
-// store this warp's 16 rows x 128 B (64 bf16 / 32 fp32 columns) starting at column col
-__device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e, const TileCoord& c, int warp, int col) {
-  if (d.a_mode == 1) {
-    const int r0 = warp * 16;
-    const int yy = r0 / d.bw, xx = r0 - yy * d.bw;
-    tma_store_4d(e.tm, e.stg_ptr, col, c.x0 + xx, c.y0 + yy, c.img);
-  } else {
-    tma_store_2d(e.tm, e.stg_ptr, col, c.m0 + warp * 16);
+// byte offset of the staging tile to fill next: the copy issued from it two blocks ago has finished reading it
+__device__ __forceinline__ int epi_stage_acquire(EpiTma& e, int lane) {
+  if (lane == 0) bulk_wait_read1();
+  __syncwarp();
+  const int off = e.cur * kXposeWarp;
+  e.cur ^= 1;
+  return off;
+}
+
+// v = this thread's 16 accumulators of columns 32k .. 32k + 31 (k uniform over the warp, k < S / 16); register indices
+// stay compile-time
+template <int S, int K = 0>
+__device__ __forceinline__ void acc_chunk(int k, const float (&a)[S], float (&v)[16]) {
+  if constexpr (K + 1 < S / 16) {
+    if (k != K) { acc_chunk<S, K + 1>(k, a, v); return; }
   }
+#pragma unroll
+  for (int i = 0; i < 16; ++i) v[i] = a[16 * K + i];
 }
 
 __device__ __forceinline__ void epi_act(const GemmDesc& d, float (&f)[16]) {
@@ -392,115 +407,105 @@ __device__ __forceinline__ void epi_act(const GemmDesc& d, float (&f)[16]) {
     for (int j = 0; j < 16; ++j) f[j] = softplus(f[j]);
   }
 }
-// acc + bias for 16 columns starting at logical column lcol (columns >= n_logical read no bias; TMA clips them)
-__device__ __forceinline__ void epi_bias(const GemmDesc& d, const uint32_t (&v)[16], int lcol, float (&f)[16]) {
-#pragma unroll
-  for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-  if (d.bias == nullptr) return;
-  if (lcol + 16 <= d.n_logical) {
-    const float4* bp = reinterpret_cast<const float4*>(d.bias + lcol);
+// p[col], p[col + 1] of a per-column vector (col even); columns >= n_logical read nothing (TMA clips them)
+__device__ __forceinline__ float2 epi_vec2(const float* p, int col, int n_logical) {
+  if (col + 1 < n_logical) return __ldg(reinterpret_cast<const float2*>(p + col));
+  return make_float2(col < n_logical ? __ldg(p + col) : 0.f, 0.f);
+}
+// One 32-column chunk in fragment layout, col = logical column of v[0]: v[4j + e] and v[4j + 2 + e] are column
+// col + 8j + e of the thread's two rows.  (acc + bias) -> activation -> * gamma, element by element.
+__device__ __forceinline__ void epi_frag(const GemmDesc& d, float (&v)[16], int col, bool scale) {
+  if (d.bias != nullptr) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const float4 b = __ldg(bp + j);
-      f[4 * j] += b.x; f[4 * j + 1] += b.y; f[4 * j + 2] += b.z; f[4 * j + 3] += b.w;
+      const float2 b = epi_vec2(d.bias, col + 8 * j, d.n_logical);
+      v[4 * j] += b.x; v[4 * j + 1] += b.y; v[4 * j + 2] += b.x; v[4 * j + 3] += b.y;
     }
-  } else {
+  }
+  epi_act(d, v);
+  if (scale) {
 #pragma unroll
-    for (int j = 0; j < 16; ++j) if (lcol + j < d.n_logical) f[j] += __ldg(d.bias + lcol + j);
+    for (int j = 0; j < 4; ++j) {
+      const float2 g = epi_vec2(d.gamma, col + 8 * j, d.n_logical);
+      v[4 * j] *= g.x; v[4 * j + 1] *= g.y; v[4 * j + 2] *= g.x; v[4 * j + 3] *= g.y;
+    }
   }
 }
 
-// bf16 output: groups of 64 columns (128-byte row segments).  Lane l holds row l & 15 and columns 16 (l >> 4) .. + 15
-// of both 32-column halves of a group, i.e. 16-byte pieces 2 (l >> 4) + {0, 1} and 4 + 2 (l >> 4) + {0, 1} of its row.
+// store this warp's 16 rows x 128 B (64 bf16 / 32 fp32 columns) starting at column col
+__device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e, const uint8_t* tile, const TileCoord& c,
+                                              int warp, int col) {
+  if (d.a_mode == 1) {
+    const int r0 = warp * 16;
+    const int yy = r0 / d.bw, xx = r0 - yy * d.bw;
+    tma_store_4d(e.tm, tile, col, c.x0 + xx, c.y0 + yy, c.img);
+  } else {
+    tma_store_2d(e.tm, tile, col, c.m0 + warp * 16);
+  }
+}
+// bf16 output: groups of 64 columns (128-byte row segments), two 32-column chunks each.  A chunk packed to bf16 is four
+// 8 x 8 matrices per 16 columns (column octet o, rows 0-7 / 8-15), written by stmatrix: lane l addresses row l & 15 of
+// octet pair member l >> 4, 16-byte piece o ^ (row & 7) of the 128-byte row (SWIZZLE_128B).
 template <int S>
 __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                        const TileCoord& c, int warp, int lane) {
-  float* buf = reinterpret_cast<float*>(e.stg_ptr);
-  const int r = lane & 15, h = lane >> 4;
-  const float* rowp = buf + r * 32;
-  const int sw = xpose16_swz(r) ^ (lane & 16);
+  const int oct = lane >> 4;
+  const uint32_t lane_off = (lane & 15) * 128;
   for (int g = 0; 64 * g < 2 * S; ++g) {
     const int lcol = c.n0 + g * 64;
     if (lcol >= d.n_logical) break;
-    if (lane == 0) bulk_wait_read0();                      // the previous copy has finished reading the staging tile
-    __syncwarp();
-    uint32_t v0[16], v1[16];
-    acc_stage16_k(2 * g, acc, buf, lane);
-    __syncwarp();
-    acc_read_row<16>(rowp, sw, v0);
-    __syncwarp();
-    acc_stage16_k(2 * g + 1, acc, buf, lane);
-    __syncwarp();
-    acc_read_row<16>(rowp, sw, v1);
-    __syncwarp();
-    float f0[16], f1[16];
-    epi_bias(d, v0, lcol + 16 * h, f0);
-    epi_bias(d, v1, lcol + 32 + 16 * h, f1);
-    epi_act(d, f0);
-    epi_act(d, f1);
-    const uint32_t row = e.stg + r * 128;
-    const int swz = r & 7;
+    const int tile = epi_stage_acquire(e, lane);
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      st_shared_v4(row + (((2 * h + j) ^ swz) << 4), pack_bf16(f0[8 * j], f0[8 * j + 1]), pack_bf16(f0[8 * j + 2], f0[8 * j + 3]),
-                   pack_bf16(f0[8 * j + 4], f0[8 * j + 5]), pack_bf16(f0[8 * j + 6], f0[8 * j + 7]));
-      st_shared_v4(row + (((4 + 2 * h + j) ^ swz) << 4), pack_bf16(f1[8 * j], f1[8 * j + 1]), pack_bf16(f1[8 * j + 2], f1[8 * j + 3]),
-                   pack_bf16(f1[8 * j + 4], f1[8 * j + 5]), pack_bf16(f1[8 * j + 6], f1[8 * j + 7]));
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { epi_tma_store(d, e, c, warp, d.out_col0 + lcol); bulk_commit(); }
-  }
-}
-
-// fp32 output (a_mode 0): chunks of 32 columns (128-byte row segments), lane l holding row l & 15, 16-byte pieces
-// 4 (l >> 4) .. + 3.  The residual-stream update x += gamma * (acc + bias) stages gamma * (acc + bias) and lets the copy
-// engine ADD it into x (cp.reduce.async.bulk.tensor .add.f32, performed in the L2): the SM never reads x.  Each element
-// is updated by exactly one tile: deterministic.
-template <int S>
-__device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
-                                                      const TileCoord& c, int warp, int lane) {
-  float* buf = reinterpret_cast<float*>(e.stg_ptr);
-  const int r = lane & 15, h = lane >> 4;
-  const float* rowp = buf + r * 32;
-  const int sw = xpose16_swz(r) ^ (lane & 16);
-  for (int ch = 0; 32 * ch < 2 * S; ++ch) {
-    const int lcol = c.n0 + ch * 32;
-    if (lcol >= d.n_logical) break;
-    if (lane == 0) bulk_wait_read0();                      // the previous copy has finished reading the staging tile
-    __syncwarp();
-    uint32_t v[16];
-    acc_stage16_k(ch, acc, buf, lane);
-    __syncwarp();
-    acc_read_row<16>(rowp, sw, v);
-    __syncwarp();
-    const int l0 = lcol + 16 * h;
-    float f[16];
-    epi_bias(d, v, l0, f);
-    epi_act(d, f);
-    if (d.gamma != nullptr) {
-      if (l0 + 16 <= d.n_logical) {
+    for (int h = 0; h < 2; ++h) {
+      float v[16];
+      acc_chunk(2 * g + h, acc, v);
+      epi_frag(d, v, lcol + 32 * h + 2 * (lane & 3), false);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float4 g = __ldg(reinterpret_cast<const float4*>(d.gamma + l0) + j);
-          f[4 * j] *= g.x; f[4 * j + 1] *= g.y; f[4 * j + 2] *= g.z; f[4 * j + 3] *= g.w;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) f[j] = l0 + j < d.n_logical ? f[j] * __ldg(d.gamma + l0 + j) : 0.f;
+      for (int p = 0; p < 2; ++p) {
+        const int o = 4 * h + 2 * p;           // octets o (lanes 0-15) and o + 1 (lanes 16-31)
+        const uint32_t addr = e.stg + tile + lane_off + (((o + oct) ^ (lane & 7)) << 4);
+        stmatrix_x4(addr, pack_bf16(v[8 * p], v[8 * p + 1]), pack_bf16(v[8 * p + 2], v[8 * p + 3]),
+                        pack_bf16(v[8 * p + 4], v[8 * p + 5]), pack_bf16(v[8 * p + 6], v[8 * p + 7]));
       }
     }
-    const uint32_t row = e.stg + r * 128;
-    const int swz = r & 7;
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      st_shared_v4(row + (((4 * h + j) ^ swz) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]),
-                   __float_as_uint(f[4 * j + 2]), __float_as_uint(f[4 * j + 3]));
     fence_proxy_async_smem();
     __syncwarp();
     if (lane == 0) {
-      if (d.gamma != nullptr) tma_reduce_add_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + warp * 16);
-      else tma_store_2d(e.tm, e.stg_ptr, d.out_col0 + lcol, c.m0 + warp * 16);
+      epi_tma_store(d, e, e.stg_ptr + tile, c, warp, d.out_col0 + lcol);
+      bulk_commit();
+    }
+  }
+}
+
+// fp32 output (a_mode 0): chunks of 32 columns (128-byte row segments).  A thread writes its column pairs as 8-byte
+// stores: pair j of row r is half (lane & 1) of 16-byte piece (2j + (lane % 4) / 2) ^ (r & 7) (rows r and r + 8 share
+// the swizzle; a half-warp's four rows meet in two pieces, a 2-way bank conflict on 8 stores per chunk).
+// The residual-stream update x += gamma * (acc + bias) stages gamma * (acc + bias) and lets the copy engine ADD it into
+// x (cp.reduce.async.bulk.tensor .add.f32, performed in the L2): the SM never reads x.  Each element is updated by
+// exactly one tile: deterministic.
+template <int S>
+__device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
+                                                      const TileCoord& c, int warp, int lane) {
+  const int r = lane >> 2, q = lane & 3;
+  const uint32_t lane_off = r * 128 + (q & 1) * 8;
+  for (int ch = 0; 32 * ch < 2 * S; ++ch) {
+    const int lcol = c.n0 + ch * 32;
+    if (lcol >= d.n_logical) break;
+    const int tile = epi_stage_acquire(e, lane);
+    float v[16];
+    acc_chunk(ch, acc, v);
+    epi_frag(d, v, lcol + 2 * q, d.gamma != nullptr);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint32_t addr = e.stg + tile + lane_off + (((2 * j + (q >> 1)) ^ r) << 4);
+      st_shared_v2f(addr, v[4 * j], v[4 * j + 1]);
+      st_shared_v2f(addr + 8 * 128, v[4 * j + 2], v[4 * j + 3]);
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      if (d.gamma != nullptr) tma_reduce_add_2d(e.tm, e.stg_ptr + tile, d.out_col0 + lcol, c.m0 + warp * 16);
+      else tma_store_2d(e.tm, e.stg_ptr + tile, d.out_col0 + lcol, c.m0 + warp * 16);
       bulk_commit();
     }
   }
@@ -574,14 +579,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord
     orow = (static_cast<long long>(img) * d.H * d.ps + y * d.ps + ky) * (d.W * d.ps) + x * d.ps + kx;
   }
   // TMA epilogue for this tile?  (the V^T tiles of the fused qkv projection keep the transposing direct store)
-  const bool tma_tile = et != nullptr && d.tma_out != 0 && !(d.vt != nullptr && c.n0 >= d.vt_col0);
-  if (tma_tile) {
-    if (d.tma_out == 1) epilogue_tile_tma_bf16(d, *et, acc, c, warp, lane);
-    else epilogue_tile_tma_f32(d, *et, acc, c, warp, lane);
+  if (et != nullptr && d.tma_out != 0 && !(d.vt != nullptr && c.n0 >= d.vt_col0)) {
+    if (d.tma_out == 2) {
+      epilogue_tile_tma_f32(d, *et, acc, c, warp, lane);
+    } else if constexpr (S % 32 == 0) {     // the host selects tma_out 1 only for widths of whole 64-column groups
+      epilogue_tile_tma_bf16(d, *et, acc, c, warp, lane);
+    }
     return;
   }
-  // In pf_gemm_kernel `buf` is also this warp's TMA staging tile: a direct-store tile (the V^T tiles of the fused qkv
-  // projection) may follow a TMA tile whose bulk copy is still reading it.
+  // In pf_gemm_kernel `buf` is also this warp's first TMA staging tile: a direct-store tile (the V^T tiles of the fused
+  // qkv projection) may follow a TMA tile whose bulk copy is still reading it.
   if (et != nullptr && d.tma_out != 0) {
     if (lane == 0) bulk_wait_read0();
     __syncwarp();
@@ -655,8 +662,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
   const GemmDesc& d = P.d;
   // 1024-B alignment is required by SWIZZLE_128B operand tiles.
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* xpose = smem + stages * stage_bytes;      // [kEpiWarps][2 KB], 1024-B aligned (stage sizes are 1 KB multiples)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kXposeWarp);
+  uint8_t* xpose = smem + stages * stage_bytes;      // [kEpiWarps][2][2 KB], 1024-B aligned (stage sizes are 1 KB multiples)
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kStageWarp);
   uint64_t* empty_bar = full_bar + stages;
 
   const int warp = threadIdx.x >> 5;
@@ -721,7 +728,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
   } else {
     // ===================== consumers (warps 0..7): wgmma mainloop + epilogue =====================
     EpiTma et;
-    et.tm = &P.tmOut; et.stg_ptr = xpose + warp * kXposeWarp; et.stg = smem_u32(et.stg_ptr);
+    et.tm = &P.tmOut; et.stg_ptr = xpose + warp * kStageWarp; et.stg = smem_u32(et.stg_ptr); et.cur = 0;
     float* buf = reinterpret_cast<float*>(et.stg_ptr);
     const uint32_t a_off = static_cast<uint32_t>((warp >> 2) * 64 * 128);   // this warpgroup's 64 rows of the A tile
     float acc[BN / 2];
@@ -1142,7 +1149,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     const KernelFn gk = gemm_kernel(tmBh != nullptr, d.block_n);
     if (gk == nullptr) return set_error("gemm: block_n %d (32, 64, 96, 128, 192 or 256)", d.block_n);
     const size_t smem = 1024 + static_cast<size_t>(gemm_stages(d.block_n)) * gemm_stage_bytes(d.block_n) +
-                        kEpiWarps * kXposeWarp + kBarBytes;
+                        kEpiWarps * kStageWarp + kBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
       // weight-multicast pairs: clusters of 2 CTAs over (m-tile pair, n-tile) work items
