@@ -175,6 +175,17 @@ int pf_crop_resize(const float* img, int32_t H, int32_t W, const int32_t* origin
  * values in [0, B)), so one call may mix tiles of different images.  tile_image == NULL: image 0 (pf_crop_resize). */
 int pf_crop_resize_batched(const float* img, int32_t H, int32_t W, const int32_t* origins, const int32_t* tile_image,
                            int32_t T, int32_t th, int32_t tw, int32_t ph, int32_t pw, float* out_planar, void* stream);
+/* One image of a mixed-geometry batch: its planar fp32 [3,H,W] pixels and the th x tw size of its tiles. */
+typedef struct pf_crop_image {
+  const float* img;
+  int32_t H, W;
+  int32_t th, tw;
+} pf_crop_image;
+/* The same over images of different sizes and tile grids: `images` is a device table of descriptors and tile t is a
+ * th x tw crop of images[tile_image[t]] at origins[t], resized to (ph, pw) with the arithmetic of
+ * pf_crop_resize_batched (equal geometry gives equal bits).  tile_image is required. */
+int pf_crop_resize_multi(const pf_crop_image* images, const int32_t* origins, const int32_t* tile_image, int32_t T,
+                         int32_t ph, int32_t pw, float* out_planar, void* stream);
 /* U-Net input cat[coarse_depth_roi, fine_depth, rgb] (patchfusion.py:269) as NHWC bf16 with `ld` channels */
 int pf_pack_unet_input(const float* coarse_depth_roi, const float* fine_depth, const float* rgb_planar, int32_t T,
                        int32_t H, int32_t W, void* out, int32_t ld, void* stream);

@@ -121,12 +121,11 @@ class BaselinePretrain(TiledModel):
     def _tile_stage(self, eng, img, geom, sizes, io_raw, io_img, blk):
         """crop+resize -> fine branch per micro-batch (a micro-batch may mix images: io_img gives each tile's, None =
         image 0); the depth (in the reused tile arena) is copied into its rows of the prediction block."""
-        from . import ops
-        H, W, h, w, ph, pw = geom
+        ph, pw = self.patch_process_shape
         s0 = 0
         for T in sizes:
             crops = eng.buf('tile.crops', (T, 3, ph, pw), torch.float32)
-            ops.crop_resize(img, io_raw[s0:s0 + T], None if io_img is None else io_img[s0:s0 + T], h, w, ph, pw, crops)
+            self._crop(img, geom, io_raw[s0:s0 + T], None if io_img is None else io_img[s0:s0 + T], crops)
             arena = eng.arena('tile', eng.branch_bytes('fine', T))
             fd, _ = eng.branch('fine', crops, ws=(arena, 0))
             blk[s0:s0 + T].copy_(fd)
@@ -135,9 +134,11 @@ class BaselinePretrain(TiledModel):
     def _compute_phase(self, eng, phase, img, geom, raw, process_num, shard):
         """Fine-branch predictions of this rank's tiles of the ordered tile list `raw` ((image, y, x) items of img
         [B,3,H,W], or (y, x) tiles of image 0) -> its block [block_rows, ph, pw] fp32 (round-robin: row j = tile
-        rank + j * world)."""
+        rank + j * world).  geom: one (H, W, h, w, ph, pw), or one per image of a mixed batch (img is then its crop
+        table)."""
         from .parallel import shard_indices, block_rows
-        H, W, h, w, ph, pw = geom
+        ph, pw = self.patch_process_shape
+        mixed = self.is_mixed(geom)
         rank, world = (0, 1) if shard is None else shard
         n = len(raw)
         own = shard_indices(n, rank, world)
@@ -147,9 +148,9 @@ class BaselinePretrain(TiledModel):
         chunk, images = self.split_tiles([raw[i] for i in own])
         io_raw = eng.buf('io.raw.' + phase, (len(own), 2), torch.int32)
         io_raw.copy_(torch.tensor(chunk, dtype=torch.int32))
-        B = img.shape[0] if img.dim() == 4 else 1
+        B = len(geom) if mixed else img.shape[0] if img.dim() == 4 else 1
         io_img = None
-        if B > 1:
+        if B > 1 or mixed:
             io_img = eng.buf('io.img.' + phase, (len(own),), torch.int32)
             io_img.copy_(torch.tensor(images, dtype=torch.int32))
         sizes = self._micro_sizes(len(own), process_num)
@@ -164,25 +165,28 @@ class BaselinePretrain(TiledModel):
         Fine target: image_hr [B,3,H,W] with any B >= 1 (extension: the reference takes B = 1) -> [B,1,H',W']; the
         tiles of all images are micro-batched together and image b equals the single-image call made after images
         0..b-1 from the same `random` state.  `shard=(rank, world)` / `('emulate', W)` shards the tile list
-        round-robin with one all-gather before the deterministic stitch (as `PatchFusion.forward`)."""
+        round-robin with one all-gather before the deterministic stitch (as `PatchFusion.forward`).  The fine target
+        also takes a mixed batch (lists of images, tile_cfgs and modes) and then returns a list, as
+        `PatchFusion.forward`; the coarse target takes one image_lr batch of one size."""
         if mode == 'train':
             raise NotImplementedError('training is out of scope of the H100 hot-path build (SURVEY.md §2 rows 10,12)')
         if self.target == 'coarse':
+            if isinstance(image_lr, (list, tuple)):
+                raise ValueError('the coarse target takes image_lr as one [B, 3, h, w] tensor, not a list')
             depth = self._coarse_infer(image_lr)
             return depth, {'rgb': image_lr, 'depth_pred': depth, 'depth_gt': depth_gt}
         if self.target != 'fine':
             raise NotImplementedError
-        if tile_cfg is None:
-            tile_cfg = self.tile_cfg
-        else:
-            tile_cfg = self.prepare_tile_cfg(tile_cfg['image_raw_shape'], tile_cfg['patch_split_num'])
-        assert image_hr.shape[0] >= 1
+        image_hr, tile_cfg, cai_mode, as_list = self._batch_inputs(image_hr, tile_cfg, cai_mode)
+        assert len(image_hr) >= 1
         self._check_shard(shard, group)
         eng = self.engine()
 
         def compute(phase, img, geom, tiles, sh, plan):
             return self._compute_phase(eng, phase, img, geom, tiles, process_num, sh)
 
-        n_calls = int(cai_mode[1:]) if cai_mode[0] == 'r' else 0      # BP:407-410: N calls, not N // process_num
+        n_calls = lambda m: int(m[1:])              # BP:407-410: N calls, not N // process_num
         depth = self._tiled_forward(eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_calls, compute)
+        if as_list and not isinstance(depth, list):
+            depth = list(depth.split(1))
         return depth, {}

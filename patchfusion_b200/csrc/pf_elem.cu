@@ -450,6 +450,35 @@ __global__ void crop_resize_kernel(const float* __restrict__ img, int H, int W, 
   out[idx] = (1.f - fy) * ((1.f - fx) * v00 + fx * v01) + fy * ((1.f - fx) * v10 + fx * v11);
 }
 
+// crop_resize_kernel over images of different sizes: tile ti reads descriptor images[tile_image[ti]] (its own planar
+// [3,H,W] image and crop size th x tw).  Same index order and bilinear arithmetic, so equal geometry gives equal bits.
+__global__ void crop_resize_multi_kernel(const pf_crop_image* __restrict__ images, const int* __restrict__ origins,
+                                         const int* __restrict__ tile_image, int T, int ph, int pw,
+                                         float* __restrict__ out) {
+  long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  long long total = static_cast<long long>(T) * 3 * ph * pw;
+  if (idx >= total) return;
+  int ox = static_cast<int>(idx % pw);
+  long long t = idx / pw;
+  int oy = static_cast<int>(t % ph);
+  t /= ph;
+  int c = static_cast<int>(t % 3);
+  int ti = static_cast<int>(t / 3);
+  const pf_crop_image d = images[tile_image[ti]];
+  const int H = d.H, W = d.W;
+  int y0, y1, x0, x1; float fy, fx;
+  ac_coord(oy, d.th, ph, y0, y1, fy);
+  ac_coord(ox, d.tw, pw, x0, x1, fx);
+  const float* base = d.img + (static_cast<long long>(c) * H + origins[ti * 2]) * W + origins[ti * 2 + 1];
+  float v00 = base[static_cast<long long>(y0) * W + x0], v01 = base[static_cast<long long>(y0) * W + x1];
+  float v10 = base[static_cast<long long>(y1) * W + x0], v11 = base[static_cast<long long>(y1) * W + x1];
+  // The blend of crop_resize_kernel with its FMA contraction spelled out (nvcc fuses the first product of each a*b + c*d
+  // there): left to the compiler, this kernel fused the other product of one row and differed in the last bit.
+  const float top = __fmaf_rn(1.f - fx, v00, __fmul_rn(fx, v01));
+  const float bot = __fmaf_rn(1.f - fx, v10, __fmul_rn(fx, v11));
+  out[idx] = __fmaf_rn(1.f - fy, top, __fmul_rn(fy, bot));
+}
+
 __global__ void pack_unet_input_kernel(const float* __restrict__ cd, const float* __restrict__ fd,
                                        const float* __restrict__ rgb, int T, int H, int W, bf16* __restrict__ out,
                                        int ld) {
@@ -1001,6 +1030,15 @@ int pf_crop_resize_batched(const float* img, int32_t H, int32_t W, const int32_t
 int pf_crop_resize(const float* img, int32_t H, int32_t W, const int32_t* origins, int32_t T, int32_t th, int32_t tw,
                    int32_t ph, int32_t pw, float* out_planar, void* stream) {
   return pf_crop_resize_batched(img, H, W, origins, nullptr, T, th, tw, ph, pw, out_planar, stream);
+}
+
+int pf_crop_resize_multi(const pf_crop_image* images, const int32_t* origins, const int32_t* tile_image, int32_t T,
+                         int32_t ph, int32_t pw, float* out_planar, void* stream) {
+  if (images == nullptr || tile_image == nullptr) return set_error("pf_crop_resize_multi: images and tile_image are required");
+  if (T <= 0) return 0;
+  long long total = static_cast<long long>(T) * 3 * ph * pw;
+  crop_resize_multi_kernel<<<nblocks(total, 256), 256, 0, ST>>>(images, origins, tile_image, T, ph, pw, out_planar);
+  return check_launch("crop_resize_multi_kernel");
 }
 
 int pf_pack_unet_input(const float* coarse_depth_roi, const float* fine_depth, const float* rgb_planar, int32_t T,

@@ -42,6 +42,11 @@ class GemmDesc(C.Structure):
     ]
 
 
+class CropImage(C.Structure):
+    """Mirror of `pf_crop_image` (include/pf_b200.h): one image of a pf_crop_resize_multi table."""
+    _fields_ = [('img', C.c_void_p), ('H', C.c_int32), ('W', C.c_int32), ('th', C.c_int32), ('tw', C.c_int32)]
+
+
 _i, _f, _p, _ll = C.c_int32, C.c_float, C.c_void_p, C.c_int64
 # name -> argument types (all return int status), in the order of include/pf_b200.h
 SIGNATURES = {
@@ -66,6 +71,7 @@ SIGNATURES = {
     'pf_im2col_3x3_s2': [_p, _i, _i, _i, _i, _i, _p, _p],
     'pf_crop_resize': [_p, _i, _i, _p, _i, _i, _i, _i, _i, _p, _p],
     'pf_crop_resize_batched': [_p, _i, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p],
+    'pf_crop_resize_multi': [_p, _p, _p, _i, _i, _i, _p, _p],
     'pf_pack_unet_input': [_p, _p, _p, _i, _i, _i, _p, _i, _p],
     'pf_f32_to_bf16': [_p, _ll, _p, _p],
     'pf_ingest_u8': [_p, _i, _i, _i, _i, _i, _p, _p],

@@ -166,8 +166,22 @@ class TiledModel(ParamTree):
     @torch.no_grad()
     def make_lr(self, image_hr):
         """`image_lr = model.resizer(image)` of `tools/test_single_forward.py:13-14` on the device (same bilinear
-        align_corners=True resample, pf_crop_resize with one whole-image tile per image): [B,3,H,W] -> [B,3,ph,pw]."""
+        align_corners=True resample, pf_crop_resize with one whole-image tile per image): [B,3,H,W] -> [B,3,ph,pw].
+        A list of B images [1,3,H_b,W_b] of different sizes (a mixed batch) gives the same [B,3,ph,pw] batch, through
+        pf_crop_resize_multi; every image must resize to the same (ph, pw)."""
         from . import ops
+        if isinstance(image_hr, (list, tuple)):
+            imgs = [x.float().contiguous() for x in image_hr]
+            sizes = sorted({self.resizer.out_size(*x.shape[-2:]) for x in imgs})
+            if len(sizes) != 1:
+                raise ValueError('make_lr: the images resize to different sizes %s' % sizes)
+            (ph, pw), B, dev = sizes[0], len(imgs), imgs[0].device
+            out = torch.empty((B, 3, ph, pw), dtype=torch.float32, device=dev)
+            table = torch.empty((ops.crop_table_bytes(B),), dtype=torch.uint8, device=dev)
+            ops.crop_table(imgs, [tuple(x.shape[-2:]) for x in imgs], table)
+            org = torch.zeros((B, 2), dtype=torch.int32, device=dev)
+            ops.crop_resize_multi(table, org, torch.arange(B, dtype=torch.int32, device=dev), ph, pw, out)
+            return out
         img = image_hr.float().contiguous()
         B = img.shape[0]
         H, W = img.shape[-2:]
@@ -260,12 +274,18 @@ class TiledModel(ParamTree):
         return outs
 
     def _draw_random_boxes(self, n_calls, process_num, H, W, h, w, shard, group, dev, n_images=1):
+        """draw_random_boxes for n_images images of one geometry, each with n_calls calls."""
+        return TiledModel.draw_random_boxes([(n_calls, H, W, h, w)] * n_images, process_num, shard, group, dev)
+
+    @staticmethod
+    def draw_random_boxes(specs, process_num, shard, group, dev):
         """Random tiles (image, y, x), image by image, each in the reference's draw order (baseline_pretrain.py:155-156:
-        process_num rows, then ONE shared column per call): the draws of B sequential single-image calls.  Under real
-        sharding rank 0's draws are broadcast once for the batch so every rank stitches the same list (all ranks still
-        advance their own `random` state identically)."""
+        process_num rows, then ONE shared column per call): the draws of B sequential single-image calls.  specs[b] =
+        (calls, H, W, h, w) of image b (calls 0: the image has no random phase).  Under real sharding rank 0's draws
+        are broadcast once for the batch so every rank stitches the same list (all ranks still advance their own
+        `random` state identically)."""
         boxes = []
-        for b in range(n_images):
+        for b, (n_calls, H, W, h, w) in enumerate(specs):
             for _ in range(n_calls):
                 ys = [random.randint(0, H - h - 1) for _ in range(process_num)]
                 x0 = random.randint(0, W - w - 1)
@@ -281,7 +301,91 @@ class TiledModel(ParamTree):
     def batch_tiles(tiles, n_images):
         """The batch's tile list: every image's tiles (y, x) in their single-image order, image-major, as
         (image, y, x).  Tile i of image b is item b * len(tiles) + i."""
-        return [(b, y, x) for b in range(n_images) for (y, x) in tiles]
+        return TiledModel.mixed_tiles([tiles] * n_images)
+
+    @staticmethod
+    def mixed_tiles(per_image):
+        """The tile list of images with tile lists of their own (per_image[b]: image b's (y, x) tiles), image-major,
+        as (image, y, x)."""
+        return [(b, y, x) for b, tiles in enumerate(per_image) for (y, x) in tiles]
+
+    @staticmethod
+    def regular_tiles(tile_cfg, cai_mode, patch_process_shape):
+        """One image's regular tiles in the reference's order (baseline_pretrain.py:221-251): raw (y, x) origins in the
+        image and the matching proc origins on the patch_reensemble canvas.  m1: the split grid; m2 and rN add the
+        three grids shifted by half a tile."""
+        H, W = tile_cfg['image_raw_shape']
+        h, w = tile_cfg['patch_raw_shape']
+        ph, pw = patch_process_shape
+        offsets = [((0, 0), (0, 0))]
+        if cai_mode == 'm2' or cai_mode[0] == 'r':
+            offsets += [((0, w // 2), (0, pw // 2)), ((h // 2, 0), (ph // 2, 0)), ((h // 2, w // 2), (ph // 2, pw // 2))]
+        raw, proc = [], []
+        for (oy, ox), (py, px) in offsets:
+            assert ox >= 0 and oy >= 0
+            ny, nx = (H - oy) // h, (W - ox) // w
+            raw += [(h * a + oy, w * b + ox) for a in range(ny) for b in range(nx)]
+            proc += [(ph * a + py, pw * b + px) for a in range(ny) for b in range(nx)]
+        return raw, proc
+
+    @staticmethod
+    def is_mixed(geom):
+        """geom is one (H, W, h, w, ph, pw) for the whole batch, or a tuple of them, one per image (a mixed batch)"""
+        return isinstance(geom[0], tuple)
+
+    @staticmethod
+    def roi_boxes(items, geoms):
+        """ROI boxes [n, 4] fp32 (x1, y1, x2, y2 in patch_process units) of (image, y, x) items, or (y, x) items of
+        image 0, exactly as baseline_pretrain.py:268-282: the integer pixel box times its image's fp32 factors
+        (geoms[b] = (H, W, h, w, ph, pw) of image b)."""
+        fac = [(np.float32(1 / W * pw), np.float32(1 / H * ph), h, w) for (H, W, h, w, ph, pw) in geoms]
+        out = np.empty((len(items), 4), dtype=np.float32)
+        for i, it in enumerate(items):
+            fx, fy, h, w = fac[it[0] if len(it) == 3 else 0]
+            y, x = it[-2:]
+            out[i] = (np.float32(x) * fx, np.float32(y) * fy, np.float32(x + w) * fx, np.float32(y + h) * fy)
+        return out
+
+    @staticmethod
+    def _crop(img, geom, raw, tile_image, out):
+        """crop + resize to out [T,3,ph,pw] of the tiles at origins `raw` ([T,2] int32) of the images tile_image ([T]
+        int32, None: image 0).  One geometry: img is the batch [B,3,H,W] (or [3,H,W]).  Mixed batch: img is the
+        pf_crop_resize_multi table of the images, which carries each image's size and tile size."""
+        from . import ops
+        if TiledModel.is_mixed(geom):
+            ops.crop_resize_multi(img, raw, tile_image, out.shape[2], out.shape[3], out)
+        else:
+            H, W, h, w, ph, pw = geom
+            ops.crop_resize(img, raw, tile_image, h, w, ph, pw, out)
+
+    def _batch_inputs(self, image_hr, tile_cfg, cai_mode):
+        """forward's image_hr / tile_cfg / cai_mode -> (image_hr, tile_cfg, cai_mode, mixed).  One geometry (a [B,3,H,W]
+        tensor, a dict or None, a string): the tensor, the prepared tile_cfg and the mode, mixed False.  A mixed batch
+        (any of the three a list; a tensor or a single tile_cfg / mode applies to every image): lists of B images
+        [1,3,H_b,W_b], prepared tile_cfgs and modes, mixed True, after the reference's per-image checks.  A mixed batch
+        whose images all share one tile_cfg and mode comes back as that tensor batch, still with mixed True (the caller
+        returns a list)."""
+        def prep(c):
+            return self.tile_cfg if c is None else self.prepare_tile_cfg(c['image_raw_shape'], c['patch_split_num'])
+        lists = [isinstance(a, (list, tuple)) for a in (image_hr, tile_cfg, cai_mode)]
+        if not any(lists):
+            return image_hr, prep(tile_cfg), cai_mode, False
+        B = len(image_hr) if lists[0] else image_hr.shape[0]
+        if B < 1:
+            raise ValueError('a mixed batch needs at least one image')
+        for a, is_list, name in ((tile_cfg, lists[1], 'tile_cfg'), (cai_mode, lists[2], 'cai_mode')):
+            if is_list and len(a) != B:
+                raise ValueError('%s holds %d entries for %d images' % (name, len(a), B))
+        images = list(image_hr) if lists[0] else list(image_hr.split(1))
+        cfgs = [prep(c) for c in (tile_cfg if lists[1] else [tile_cfg] * B)]
+        modes = list(cai_mode) if lists[2] else [cai_mode] * B
+        for x, cfg in zip(images, cfgs):
+            assert x.dim() == 4 and x.shape[:2] == (1, 3), 'every image of a mixed batch must be [1, 3, H, W]'
+            assert tuple(x.shape[-2:]) == tuple(cfg['image_raw_shape']), 'image_hr must already be at image_raw_shape'
+        keys = {(tuple(c['image_raw_shape']), tuple(c['patch_split_num']), m) for c, m in zip(cfgs, modes)}
+        if len(keys) == 1:
+            return torch.cat(images), cfgs[0], modes[0], True
+        return images, cfgs, modes, True
 
     @staticmethod
     def image_ranges(items, n_images):
@@ -301,66 +405,76 @@ class TiledModel(ParamTree):
 
     def _tiled_forward(self, eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_random_calls, compute,
                        image_lr=None, plan_fn=None):
-        """Tiled inference of a batch of B images sharing one tile_cfg: the regular passes
-        (baseline_pretrain.py:221-331, patchfusion.py:417-439) are independent tiles whose stitch is a weighted sum, so
-        all passes of all images are flattened into one ordered, image-major tile list of (image, y, x) and
-        micro-batched (a micro-batch may mix images); rN modes then resize each canvas to image_raw_shape and add
-        `n_random_calls` calls of `process_num` random tiles per image.  The stitch runs once per image over that
-        image's part of the list, so image b's canvas equals its single-image run bit for bit.  image_lr (PatchFusion)
-        goes into its static buffer; plan_fn(n) gives the rank of each regular tile (None: round-robin)."""
+        """Tiled inference of a batch of B images: the regular passes (baseline_pretrain.py:221-331,
+        patchfusion.py:417-439) are independent tiles whose stitch is a weighted sum, so all passes of all images are
+        flattened into one ordered, image-major tile list of (image, y, x) and micro-batched (a micro-batch may mix
+        images); rN modes then resize each canvas to image_raw_shape and add n_random_calls(mode) calls of
+        `process_num` random tiles per image.  The stitch runs once per image over that image's part of the list, so
+        image b's canvas equals its single-image run bit for bit.
+        One geometry: image_hr [B,3,H,W], one prepared tile_cfg and mode -> depth [B,1,H',W'].  Mixed batch (see
+        _batch_inputs): lists of B images [1,3,H_b,W_b], tile_cfgs and modes -> a list of B depths [1,1,H'_b,W'_b];
+        each image gets its own static buffer and the crops read them through one pf_crop_resize_multi table.
+        image_lr (PatchFusion) goes into its static buffer; plan_fn(n) gives the rank of each regular tile (None:
+        round-robin)."""
         from . import ops
         from .parallel import slot_table
-        dev = image_hr.device
-        B = image_hr.shape[0]
-        H, W = tile_cfg['image_raw_shape']
-        assert tuple(image_hr.shape[-2:]) == (H, W), 'image_hr must already be at image_raw_shape'
-        h, w = tile_cfg['patch_raw_shape']
+        mixed = isinstance(image_hr, list)
+        B = len(image_hr) if mixed else image_hr.shape[0]
+        cfgs = tile_cfg if mixed else [tile_cfg] * B
+        modes = cai_mode if mixed else [cai_mode] * B
+        dev = image_hr[0].device
         ph, pw = self.patch_process_shape
-        RH, RW = tile_cfg['patch_reensemble_shape']
-        geom = (H, W, h, w, ph, pw)
+        geoms = [tuple(c['image_raw_shape']) + tuple(c['patch_raw_shape']) + (ph, pw) for c in cfgs]
         world = 1 if shard is None else shard[1]
         # inputs into static buffers (stable addresses for the captured graphs)
-        img = eng.buf('in.image_hr', (B, 3, H, W), torch.float32)
-        img.copy_(image_hr)
+        if mixed:
+            bufs = [eng.buf('in.image_hr.%d' % b, (1, 3) + g[:2], torch.float32) for b, g in enumerate(geoms)]
+            for buf, x in zip(bufs, image_hr):
+                assert tuple(x.shape[-2:]) == buf.shape[-2:], 'image_hr must already be at image_raw_shape'
+                buf.copy_(x)
+            img = ops.crop_table(bufs, [g[2:4] for g in geoms],
+                                 eng.buf('in.crop_table', (ops.crop_table_bytes(B),), torch.uint8))
+            geom = tuple(geoms)
+        else:
+            geom = geoms[0]
+            assert tuple(image_hr.shape[-2:]) == geom[:2], 'image_hr must already be at image_raw_shape'
+            img = eng.buf('in.image_hr', (B, 3) + geom[:2], torch.float32)
+            img.copy_(image_hr)
         if image_lr is not None:
             assert image_lr.shape[0] == B, 'image_lr and image_hr must hold the same number of images'
             eng.buf('in.image_lr', (B, 3, ph, pw), torch.float32).copy_(image_lr)
         mask = self._mask((ph, pw), dev)
-        offsets = [((0, 0), (0, 0))]
-        if cai_mode == 'm2' or cai_mode[0] == 'r':
-            offsets += [((0, w // 2), (0, pw // 2)), ((h // 2, 0), (ph // 2, 0)), ((h // 2, w // 2), (ph // 2, pw // 2))]
-        raw, proc = [], []
-        for (oy, ox), (py, px) in offsets:
-            assert ox >= 0 and oy >= 0
-            ny, nx = (H - oy) // h, (W - ox) // w
-            raw += [(h * a + oy, w * b + ox) for a in range(ny) for b in range(nx)]
-            proc += [(ph * a + py, pw * b + px) for a in range(ny) for b in range(nx)]
-        is_r = cai_mode[0] == 'r'
-        tiles = self.batch_tiles(raw, B)
+        raws, procs = zip(*[self.regular_tiles(c, m, (ph, pw)) for c, m in zip(cfgs, modes)])
+        is_r = [m[0] == 'r' for m in modes]
+        tiles = self.mixed_tiles(raws)
         plan = plan_fn(len(tiles)) if plan_fn is not None else None
         full = self._exchange(lambda sh: compute('reg', img, geom, tiles, sh, plan), shard, group)
         slots = slot_table(len(tiles), world, plan)
-        n = len(raw)
-        CH, CW = (H, W) if is_r else (RH, RW)
-        depth = torch.empty((B, 1, CH, CW), dtype=torch.float32, device=dev)
-        bases = []
-        for b in range(B):
-            outs = self._stitch_phase(eng, 'reg', full, proc, slots[b * n:(b + 1) * n], ph, pw, mask, (0, 0), None,
-                                      (RH, RW), ('num', 'den') if is_r else ('avg',), avg_out=depth[b, 0])
-            if is_r:
+        sizes = [g[:2] if r else tuple(c['patch_reensemble_shape']) for g, c, r in zip(geoms, cfgs, is_r)]
+        if mixed:
+            depth = [torch.empty((1, 1) + s, dtype=torch.float32, device=dev) for s in sizes]
+        else:
+            depth = torch.empty((B, 1) + sizes[0], dtype=torch.float32, device=dev)
+        canvas = [d[0] for d in depth] if not mixed else [d[0, 0] for d in depth]      # image b's [H', W'] output
+        bases = [None] * B
+        for b, (i0, i1) in enumerate(self.image_ranges(tiles, B)):
+            H, W = geoms[b][:2]
+            RH, RW = cfgs[b]['patch_reensemble_shape']
+            outs = self._stitch_phase(eng, 'reg', full, procs[b], slots[i0:i1], ph, pw, mask, (0, 0), None,
+                                      (RH, RW), ('num', 'den') if is_r[b] else ('avg',), avg_out=canvas[b])
+            if is_r[b]:
                 n2 = torch.empty((H, W), dtype=torch.float32, device=dev)
                 d2 = torch.empty_like(n2)
                 ops.call('pf_stitch_resize', outs['num'], outs['den'], RH, RW, H, W, n2, d2, ops.stream_ptr())
-                bases.append((n2, d2))
-        if not is_r:
+                bases[b] = (n2, d2)
+        if not any(is_r):
             return depth
-        boxes = self._draw_random_boxes(n_random_calls, process_num, H, W, h, w, shard, group, dev, B)
-        if not boxes:
-            for b, (n2, d2) in enumerate(bases):
-                torch.div(n2, d2, out=depth[b, 0])
-            return depth
-        mask_r = self._mask((h, w), dev)
-        last_of = [r[1] for r in self.image_ranges(boxes, B)]     # end of each image's random tiles
+        specs = [(n_random_calls(m) if r else 0,) + g[:4] for m, r, g in zip(modes, is_r, geoms)]
+        boxes = self.draw_random_boxes(specs, process_num, shard, group, dev)
+        ranges = self.image_ranges(boxes, B)
+        for b in range(B):
+            if is_r[b] and ranges[b][0] == ranges[b][1]:        # rN with no random call: the resized canvas
+                torch.div(bases[b][0], bases[b][1], out=canvas[b])
         for s0, s1 in self._chunks(len(boxes), self.random_chunk):
             part = boxes[s0:s1]
             full = self._exchange(lambda sh: compute('rnd', img, geom, part, sh, None), shard, group)
@@ -368,10 +482,11 @@ class TiledModel(ParamTree):
             for b, (i0, i1) in enumerate(self.image_ranges(part, B)):
                 if i0 == i1:
                     continue
-                last = s0 + i1 == last_of[b]
+                H, W, h, w = geoms[b][:4]
+                last = s0 + i1 == ranges[b][1]
                 outs = self._stitch_phase(eng, 'rnd', full, [t[1:] for t in part[i0:i1]], slots[i0:i1], ph, pw,
-                                          mask_r, (h, w), bases[b], (H, W), ('avg',) if last else ('num', 'den'),
-                                          avg_out=depth[b, 0])
+                                          self._mask((h, w), dev), (h, w), bases[b], (H, W),
+                                          ('avg',) if last else ('num', 'den'), avg_out=canvas[b])
                 if not last:
                     bases[b] = (outs['num'], outs['den'])
         return depth
@@ -613,11 +728,10 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
 
     def _fine_stage(self, eng, img, T, geom, raw, tile_image=None):
         """crop+resize -> fine branch for the T tiles whose raw origins are the device rows `raw` ([T,2] int32) of the
-        images tile_image ([T] int32, None: image 0) of img ([B,3,H,W] or [3,H,W])."""
-        from . import ops
-        H, W, h, w, ph, pw = geom
+        images tile_image ([T] int32, None: image 0) of img ([B,3,H,W] or [3,H,W], or a mixed batch's crop table)."""
+        ph, pw = self.patch_process_shape
         crops = eng.buf('tile.crops', (T, 3, ph, pw), torch.float32)
-        ops.crop_resize(img, raw, tile_image, h, w, ph, pw, crops)
+        self._crop(img, geom, raw, tile_image, crops)
         # ONE arena for the tile stages, sized for the largest micro-batch: [fine branch | fusion]
         nb = (eng.branch_bytes('fine', T) + 255) // 256 * 256
         arena = eng.arena('tile', nb + eng.fusion_bytes(T, self._coarse[2]))
@@ -672,9 +786,11 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
 
     def _compute_phase(self, eng, phase, lr, img, geom, raw, process_num, shard, plan=None, group=None):
         """Fused predictions of this rank's tiles of the (global, ordered) tile list `raw` ((image, y, x) items) ->
-        its block [block_rows, ph, pw] fp32 (row j = the j-th tile of the list that `plan` gives to this rank)."""
+        its block [block_rows, ph, pw] fp32 (row j = the j-th tile of the list that `plan` gives to this rank).
+        geom: one (H, W, h, w, ph, pw), or one per image of a mixed batch (img is then its crop table)."""
         from .parallel import shard_indices, block_rows
-        H, W, h, w, ph, pw = geom
+        ph, pw = self.patch_process_shape
+        mixed = self.is_mixed(geom)
         rank, world = (0, 1) if shard is None else shard
         B = lr.shape[0]
         n = len(raw)
@@ -699,18 +815,16 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             return blk
         io_raw = eng.buf('io.raw.' + phase, (len(own), 2), torch.int32)
         io_box = eng.buf('io.box.' + phase, (len(own), 4), torch.float32)
-        fx, fy = np.float32(1 / W * pw), np.float32(1 / H * ph)
-        chunk, images = self.split_tiles([raw[i] for i in own])
+        items = [raw[i] for i in own]
+        chunk, images = self.split_tiles(items)
         io_raw.copy_(torch.tensor(chunk, dtype=torch.int32))
         io_img = None
-        if B > 1:
+        if B > 1 or mixed:
             io_img = eng.buf('io.img.' + phase, (len(own),), torch.int32)
             io_img.copy_(torch.tensor(images, dtype=torch.int32))
-        # boxes exactly as baseline_pretrain.py:268-282: int pixel box * fp32 factor
-        io_box.copy_(torch.from_numpy(np.array(
-            [[np.float32(x) * fx, np.float32(y) * fy, np.float32(x + w) * fx, np.float32(y + h) * fy]
-             for (y, x) in chunk], dtype=np.float32)))
+        io_box.copy_(torch.from_numpy(self.roi_boxes(items, geom if mixed else [geom] * B)))
         sizes = self._micro_sizes(len(own), process_num)
+        # a mixed batch's key holds every image's geometry; the modes only change tile counts, which `sizes` holds
         key = ('image', phase, tuple(sizes), blk.shape[0], with_coarse, B, self._coarse_src) + tuple(geom)
         run = lambda part: self._graphed(key + (part,), lambda: self._image_stage(
             eng, lr, img, geom, sizes, io_raw, io_box, io_img, blk, with_coarse, part))
@@ -732,14 +846,15 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         `shard=(rank, world)` (extension): this rank runs its share of the flattened tile list and ONE all-gather of
         the per-rank prediction blocks (patchfusion_b200/parallel.py) precedes the deterministic stitch, so the canvas
         is bit-identical to the single-device one.  `group`: the process group of `world` ranks (default group if
-        None).  shard=None reproduces the reference's single-device behaviour."""
+        None).  shard=None reproduces the reference's single-device behaviour.
+        Mixed batch (extension): image_hr a list of B images [1,3,H_b,W_b], each at its own image_raw_shape, tile_cfg a
+        list of B dicts and cai_mode a string or a list of B modes; process_num is shared.  image_lr stays
+        [B,3,ph,pw].  Returns a list of B depths [1,1,H'_b,W'_b] (info['depth_pred'] is that list) under the same
+        contract: image b equals the single-image call on it made after images 0..b-1."""
         if mode == 'train':
             raise NotImplementedError('training is out of scope of the H100 hot-path build (SURVEY.md §2 rows 10,12)')
-        if tile_cfg is None:
-            tile_cfg = self.tile_cfg
-        else:
-            tile_cfg = self.prepare_tile_cfg(tile_cfg['image_raw_shape'], tile_cfg['patch_split_num'])
-        B = image_hr.shape[0]
+        image_hr, tile_cfg, cai_mode, as_list = self._batch_inputs(image_hr, tile_cfg, cai_mode)
+        B = len(image_hr) if isinstance(image_hr, list) else image_hr.shape[0]
         assert B >= 1 and image_lr.shape[0] == B, 'image_lr and image_hr must hold the same number (>= 1) of images'
         self._check_shard(shard, group)
         eng = self.engine()
@@ -756,7 +871,9 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             return self._compute_phase(eng, phase, lr, img, geom, tiles, process_num, sh, plan, group)
 
         # patchfusion.py:441-448: N // process_num calls of process_num random tiles
-        n_calls = int(cai_mode[1:]) // process_num if cai_mode[0] == 'r' else 0
+        n_calls = lambda m: int(m[1:]) // process_num
         depth = self._tiled_forward(eng, image_hr, tile_cfg, cai_mode, process_num, shard, group, n_calls, compute,
                                     image_lr=image_lr, plan_fn=plan_fn)
+        if as_list and not isinstance(depth, list):
+            depth = list(depth.split(1))
         return depth, {'rgb': image_lr, 'depth_pred': depth, 'depth_gt': depth_gt}

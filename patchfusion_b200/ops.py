@@ -185,6 +185,29 @@ def crop_resize(img, origins, tile_image, th, tw, ph, pw, out):
     call('pf_crop_resize_batched', img, H, W, origins, tile_image, origins.shape[0], th, tw, ph, pw, out, stream_ptr())
 
 
+def crop_table(images, sizes, out):
+    """Write the pf_crop_resize_multi descriptors of `images` (each a contiguous fp32 [1,3,H,W] or [3,H,W] device
+    tensor) with tiles of sizes[b] = (th, tw) into `out`, a uint8 device tensor of len(images) descriptors."""
+    arr = (lib.CropImage * len(images))()
+    for d, img, (th, tw) in zip(arr, images, sizes):
+        assert img.dtype == torch.float32 and img.is_cuda and img.is_contiguous() and img.shape[-3] == 3
+        assert 0 < th <= img.shape[-2] and 0 < tw <= img.shape[-1]
+        d.img, (d.H, d.W), d.th, d.tw = img.data_ptr(), img.shape[-2:], th, tw
+    assert out.dtype == torch.uint8 and out.numel() == C.sizeof(arr)
+    out.copy_(torch.frombuffer(bytearray(arr), dtype=torch.uint8))
+    return out
+
+
+def crop_table_bytes(n):
+    return n * C.sizeof(lib.CropImage)
+
+
+def crop_resize_multi(table, origins, tile_image, ph, pw, out):
+    """Tiles of images of different sizes: tile t is a crop of the image of descriptor tile_image[t] of `table`
+    (crop_table) at origins[t] (int32 [T,2] device, y, x), resized to out [T,3,ph,pw] (bilinear, align_corners=True)."""
+    call('pf_crop_resize_multi', table, origins, tile_image, origins.shape[0], ph, pw, out, stream_ptr())
+
+
 def maxpool2(x, C_, out):
     B, H, W, ld = x.shape
     call('pf_maxpool2', x, B, H, W, pad_to(C_, 8), ld, out, out.shape[-1], stream_ptr())

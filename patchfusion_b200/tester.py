@@ -51,13 +51,15 @@ class Tester:
     def run(self, samples, cai_mode='m1', process_num=4, image_raw_shape=(2160, 3840), patch_split_num=(4, 4),
             batch_size=1):
         """samples: iterable of dicts {'img_file_basename': str, 'image_u8': HxWx3 uint8 BGR (cv2.imread) OR
-        'image_hr': (1,3,H,W) fp32 in [0,1], optional 'depth_gt' (1,1,h,w), optional 'boundary'}.
-        batch_size > 1: consecutive samples go through the model together (one batched forward); outputs, files and
-        metrics are those of batch_size 1, in input order.
+        'image_hr': (1,3,H,W) fp32 in [0,1], optional 'depth_gt' (1,1,h,w), optional 'boundary', optional 'tile_cfg'
+        ({'image_raw_shape', 'patch_split_num'}) and 'cai_mode'}.  A sample without its own tile_cfg / cai_mode uses
+        the run's (image_raw_shape, patch_split_num, cai_mode).
+        batch_size > 1: consecutive samples go through the model together (one batched forward; samples of different
+        geometry or mode form a mixed batch); outputs, files and metrics are those of batch_size 1, in input order.
         Returns the list of per-image metric dicts (empty when no ground truth is given)."""
         model = self.model
         dev = next(model.parameters()).device
-        tile_cfg = {'image_raw_shape': list(image_raw_shape), 'patch_split_num': list(patch_split_num)}
+        default_cfg = {'image_raw_shape': list(image_raw_shape), 'patch_split_num': list(patch_split_num)}
         results = []
         copy_stream = torch.cuda.Stream(device=dev)
         slots, q, th = [None, None], None, None
@@ -67,18 +69,26 @@ class Tester:
             th.start()
         i = 0
         for group in self._groups(samples, max(1, int(batch_size))):
+            cfgs = [s.get('tile_cfg', default_cfg) for s in group]
+            modes = [s.get('cai_mode', cai_mode) for s in group]
             images = []
-            for s in group:
+            for s, cfg in zip(group, cfgs):
                 if 'image_hr' in s:
                     images.append(s['image_hr'].to(dev, non_blocking=True).float())
                 else:
-                    images.append(imageio.ingest(s['image_u8'], tuple(image_raw_shape), dev, bgr=True))
-            image = images[0] if len(images) == 1 else torch.cat(images)
-            lr = model.make_lr(image)
-            results_b, _ = model(mode='infer', cai_mode=cai_mode, process_num=process_num, tile_cfg=tile_cfg,
-                                 image_lr=lr, image_hr=image)
+                    images.append(imageio.ingest(s['image_u8'], tuple(cfg['image_raw_shape']), dev, bgr=True))
+            keys = {(tuple(c['image_raw_shape']), tuple(c['patch_split_num']), m) for c, m in zip(cfgs, modes)}
+            if len(keys) == 1:
+                image = images[0] if len(images) == 1 else torch.cat(images)
+                lr = model.make_lr(image)
+                results_b, _ = model(mode='infer', cai_mode=modes[0], process_num=process_num, tile_cfg=cfgs[0],
+                                     image_lr=lr, image_hr=image)
+                results_b = [results_b[j:j + 1] for j in range(len(group))]
+            else:
+                results_b, _ = model(mode='infer', cai_mode=modes, process_num=process_num, tile_cfg=cfgs,
+                                     image_lr=model.make_lr(images), image_hr=images)
             for j, s in enumerate(group):
-                result = results_b[j:j + 1]
+                result = results_b[j]
                 self._emit(s, i, result, slots, q, copy_stream, dev, results)
                 i += 1
         if self.save:
