@@ -37,7 +37,8 @@ long long pf_launch_count(void);
  * events (duration i = event i - event i-1).  pf_profile_stop returns the record count; pf_profile_get returns a
  * record's kernel name, shape label, algorithmic flops (0 for HBM kernels) and milliseconds. */
 /* Tuning switches (defaults in parentheses; each is also read once from the environment variable of the same name):
- *   PF_OPT_TMA_EPILOGUE (1)   pf_gemm_kernel epilogue through shared memory + bulk tensor stores / reduce-add
+ *   PF_OPT_TMA_EPILOGUE (1)   pf_gemm_kernel and pf_conv3_halo_kernel epilogue through shared memory + bulk tensor
+ *                             stores / reduce-add
  *   PF_OPT_HALO_MULTICAST (1) pf_conv3_halo_kernel in clusters of 2 (value 1) or 4 (value 2) CTAs sharing the weight
  *                             tiles by TMA multicast
  *   PF_OPT_GEMM_MULTICAST (1) the same for the linear layers of pf_gemm_kernel
@@ -58,9 +59,9 @@ int pf_set_option(int32_t option, int32_t value);
 int pf_profile_start(void* stream);
 int pf_profile_stop(void);
 int pf_profile_get(int32_t i, const char** name, const char** label, double* flops, float* ms);
-/* pf_gemm_kernel phase timeline, in libraries built with -DPF_GEMM_TIMELINE (any other build returns an error):
- * synchronises the device, copies the PF_GEMM_TIMELINE_SLOTS clock64 sums accumulated by every pf_gemm_kernel launch
- * since the last reset into host array `out` (may be NULL) and zeroes them if `reset`.  Slots: producer tiles, producer
+/* pf_gemm_kernel / pf_conv3_halo_kernel phase timeline, in libraries built with -DPF_GEMM_TIMELINE (any other build
+ * returns an error): synchronises the device, copies the PF_GEMM_TIMELINE_SLOTS clock64 sums accumulated by every launch
+ * of either kernel since the last reset into host array `out` (may be NULL) and zeroes them if `reset`.  Slots: producer tiles, producer
  * cycles waiting for an empty stage, producer loop cycles; then per consumer warpgroup: tiles, cycles waiting for a
  * full stage, mainloop cycles (waits included), epilogue cycles, loop cycles. */
 #define PF_GEMM_TIMELINE_SLOTS 8

@@ -139,8 +139,12 @@ static int encode(CUtensorMap* out, const void* ptr, int rank, const uint64_t* d
     gstr[i] = strides_bytes[i];
     if (gstr[i] & 15) return set_error("tensor map: stride %d (%llu B) not a multiple of 16", i, (unsigned long long)gstr[i]);
   }
+  // rows of 128 bytes: SWIZZLE_128B (every operand tile and most staging tiles); rows of 64 bytes (the 32-column bf16
+  // staging tiles of the halo conv epilogue): SWIZZLE_64B.  The box is part of the cache key, so the mode is too.
+  const uint32_t row_bytes = box[0] * (dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2);
+  const CUtensorMapSwizzle swz = row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = fn(out, dt, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     return set_error("cuTensorMapEncodeTiled failed (%d): rank %d dims %llu %llu %llu %llu box %u %u %u %u", (int)r, rank,
@@ -461,8 +465,10 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   const bool mc = cl > 1;
   CUtensorMap tmBh;
   if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)) return 1;
-  // Epilogue through shared memory + TMA (pf_gemm_kernel only): plain bf16 outputs in 64-column groups, fp32 outputs
-  // and the fp32 residual stream (x += gamma * v) in 32-column chunks.  PF_OPT_TMA_EPILOGUE = 0 keeps the direct stores.
+  // Epilogue through shared memory + TMA: plain bf16 outputs in 64-column groups (32-column groups in the halo kernel at
+  // block_n 32), and, in pf_gemm_kernel only, fp32 outputs and the fp32 residual stream (x += gamma * v) in 32-column
+  // chunks.  Halo convs reading a fused resample keep the direct stores.  PF_OPT_TMA_EPILOGUE = 0 keeps the direct
+  // stores everywhere.
   const bool no_tma_epi = option(PF_OPT_TMA_EPILOGUE) == 0;
   CUtensorMap tmOut;
   d.tma_out = 0;
@@ -470,17 +476,19 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   // the staged zeros of columns N .. written over what the caller keeps there, so such outputs take the direct stores.
   const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;
   const bool ends16 = ocols % (d.out_f32 ? 4 : 8) == 0;
-  if (!no_tma_epi && !halo && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
-    // each consumer warp stores its 16 rows in whole 64-column groups (bf16) / 32-column chunks (fp32)
-    if (!d.out_f32 && bn % 64 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
+  if (!no_tma_epi && !(halo && any_rs) && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
+    // each consumer warp stores its 16 rows in whole column groups (bf16) / 32-column chunks (fp32)
+    const uint32_t group = halo && bn == 32 ? 32 : 64;
+    if (!d.out_f32 && bn % group == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
       if (u->a_mode == 0) {
         if (tmap_2d_bf16(&tmOut, u->out, ocols, u->M, u->out_ld, 64, 16)) return 1;
       } else {
+        // the halo kernel's 16 x 8 pixel tile: {group, 8, 2} boxes, one per consumer warp
         const uint32_t bwx = d.bw < 16 ? d.bw : 16;
-        if (tmap_4d_nhwc_bf16(&tmOut, u->out, ocols, u->W, u->H, u->NB, u->out_ld, 64, bwx, 16 / bwx)) return 1;
+        if (tmap_4d_nhwc_bf16(&tmOut, u->out, ocols, u->W, u->H, u->NB, u->out_ld, group, bwx, 16 / bwx)) return 1;
       }
       d.tma_out = 1;
-    } else if (d.out_f32 && u->a_mode == 0 && u->out_ld % 4 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
+    } else if (d.out_f32 && u->a_mode == 0 &&u->out_ld % 4 == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {
       if (tmap_2d_f32(&tmOut, u->out, ocols, u->M, u->out_ld, 32, 16)) return 1;
       d.tma_out = 2;
     }

@@ -49,9 +49,9 @@ constexpr int kGemmThreads = (kEpiWarps + 1) * 32;
 constexpr int kHaloThreads = (kEpiWarps + 3) * 32;
 constexpr int kRsWarp0 = kEpiWarps;                         // halo kernel: warps 8, 9 = resample producers
 constexpr int kMaxSmem = 227 * 1024;
-// per consumer warp: the 16 x 32 fp32 accumulator transpose of the row-per-thread epilogue.  pf_gemm_kernel has two such
-// blocks per warp, the staging tiles of the TMA-store epilogue (16 rows x 128 B, SWIZZLE_128B) used in turn; the first
-// doubles as the transpose block
+// per consumer warp: the 16 x 32 fp32 accumulator transpose of the row-per-thread epilogue.  Both kernels have two such
+// blocks per warp, the staging tiles of the TMA-store epilogue (16 rows x 128 B, SWIZZLE_128B, or x 64 B, SWIZZLE_64B)
+// used in turn; the first doubles as the transpose block
 constexpr int kXposeWarp = 16 * 32 * 4;
 constexpr int kStageWarp = 2 * kXposeWarp;
 constexpr int kBarBytes = 512;
@@ -443,27 +443,31 @@ __device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e
     tma_store_2d(e.tm, tile, col, c.m0 + warp * 16);
   }
 }
-// bf16 output: groups of 64 columns (128-byte row segments), two 32-column chunks each.  A chunk packed to bf16 is four
-// 8 x 8 matrices per 16 columns (column octet o, rows 0-7 / 8-15), written by stmatrix: lane l addresses row l & 15 of
-// octet pair member l >> 4, 16-byte piece o ^ (row & 7) of the 128-byte row (SWIZZLE_128B).
-template <int S>
+// bf16 output: groups of G = 64 columns (128-byte row segments, SWIZZLE_128B), or of G = 32 (64-byte row segments,
+// SWIZZLE_64B: the halo kernel at BN = 32), G / 32 chunks of 32 columns each.  A chunk packed to bf16 is four 8 x 8
+// matrices per 16 columns (column octet o, rows 0-7 / 8-15), written by stmatrix: lane l addresses row r = l & 15 of
+// octet pair member l >> 4, 16-byte piece o ^ (r & 7) of the 128-byte row, or o ^ ((r >> 1) & 3) of the 64-byte row
+// (the swizzle XORs address bits 4-6 with bits 7-9, or bits 4-5 with bits 7-8).
+template <int G, int S>
 __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                        const TileCoord& c, int warp, int lane) {
+  static_assert(G == 64 || G == 32, "group width");
   const int oct = lane >> 4;
-  const uint32_t lane_off = (lane & 15) * 128;
-  for (int g = 0; 64 * g < 2 * S; ++g) {
-    const int lcol = c.n0 + g * 64;
+  const uint32_t lane_off = (lane & 15) * (2 * G);
+  const int swz = G == 64 ? (lane & 7) : ((lane >> 1) & 3);
+  for (int g = 0; G * g < 2 * S; ++g) {
+    const int lcol = c.n0 + g * G;
     if (lcol >= d.n_logical) break;
     const int tile = epi_stage_acquire(e, lane);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int h = 0; h < G / 32; ++h) {
       float v[16];
-      acc_chunk(2 * g + h, acc, v);
+      acc_chunk(G / 32 * g + h, acc, v);
       epi_frag(d, v, lcol + 32 * h + 2 * (lane & 3), false);
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
         const int o = 4 * h + 2 * p;           // octets o (lanes 0-15) and o + 1 (lanes 16-31)
-        const uint32_t addr = e.stg + tile + lane_off + (((o + oct) ^ (lane & 7)) << 4);
+        const uint32_t addr = e.stg + tile + lane_off + (((o + oct) ^ swz) << 4);
         stmatrix_x4(addr, pack_bf16(v[8 * p], v[8 * p + 1]), pack_bf16(v[8 * p + 2], v[8 * p + 3]),
                         pack_bf16(v[8 * p + 4], v[8 * p + 5]), pack_bf16(v[8 * p + 6], v[8 * p + 7]));
       }
@@ -583,7 +587,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmDesc& d, const TileCoord
     if (d.tma_out == 2) {
       epilogue_tile_tma_f32(d, *et, acc, c, warp, lane);
     } else if constexpr (S % 32 == 0) {     // the host selects tma_out 1 only for widths of whole 64-column groups
-      epilogue_tile_tma_bf16(d, *et, acc, c, warp, lane);
+      epilogue_tile_tma_bf16<64>(d, *et, acc, c, warp, lane);
     }
     return;
   }
@@ -625,11 +629,13 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Phase timeline of pf_gemm_kernel (built only with -DPF_GEMM_TIMELINE; pf_gemm_timeline reads it).  One lane per
-// role records clock64 intervals in registers and adds them to g_gemm_timeline when its CTA retires: the producer
-// (slots 0-2: tiles, cycles waiting for an empty stage, cycles in its loop) and lane 0 of each consumer warpgroup's
-// first warp (slots 3-7: tiles, cycles waiting for a full stage, mainloop cycles including those waits, epilogue
-// cycles, cycles in its loop).  Every other build compiles the stamps to nothing.
+// Phase timeline of pf_gemm_kernel and pf_conv3_halo_kernel (built only with -DPF_GEMM_TIMELINE; pf_gemm_timeline reads
+// it).  One lane per role records clock64 intervals in registers and adds them to g_gemm_timeline when its CTA retires:
+// the TMA producer (slots 0-2: tiles, cycles waiting for an empty stage - halo slot or weight stage in the halo kernel -,
+// cycles in its loop) and lane 0 of each consumer warpgroup's first warp (slots 3-7: tiles, cycles waiting for a full
+// stage / halo slot, mainloop cycles including those waits, epilogue cycles, cycles in its loop).  Both kernels add to
+// the same slots: a reader takes the sums around launches of one kernel and shape.  Every other build compiles the
+// stamps to nothing.
 #ifdef PF_GEMM_TIMELINE
 constexpr int kTimelineSlots = 8;
 __device__ unsigned long long g_gemm_timeline[kTimelineSlots];
@@ -798,8 +804,8 @@ constexpr int kHaloW = 10, kHaloH = 18;
 constexpr int kHaloBytes = kHaloW * kHaloH * 128;          // 23040
 constexpr int kHaloSlot = 24 * 1024;                        // 1024-B aligned slot
 constexpr int kHaloSlots = 3;
-// shared memory left for the weight ring next to the halo slots, transposes and barriers
-constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kXposeWarp - kHaloSlots * kHaloSlot;
+// shared memory left for the weight ring next to the halo slots, the epilogue staging tiles and barriers
+constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kStageWarp - kHaloSlots * kHaloSlot;
 // taps per weight stage: amortise the per-stage barrier round trip over several taps while two stages still fit
 __host__ __device__ constexpr int halo_kc(int bn) {
   return 2 * 9 * bn * kBlockK * 2 <= kHaloBBytes ? 9 : (2 * 3 * bn * kBlockK * 2 <= kHaloBBytes ? 3 : 1);
@@ -808,6 +814,10 @@ __host__ __device__ constexpr int halo_kc(int bn) {
 __host__ __device__ constexpr int halo_stages(int bn) {
   return kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) < 6 ? kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) : 6;
 }
+// The second staging tile per warp costs no weight stage and no taps per stage at any width
+static_assert(halo_kc(32) == 9 && halo_stages(32) == 3 && halo_kc(64) == 3 && halo_stages(64) == 5 &&
+                  halo_kc(128) == 3 && halo_stages(128) == 2 && halo_kc(192) == 1 && halo_stages(192) == 5,
+              "halo weight ring");
 
 
 // ---- fused bilinear resample (align_corners=True) of a halo-kernel source -------------------------------------------
@@ -890,8 +900,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
   const GemmDesc& d = P.d;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_b = smem + kHaloSlots * kHaloSlot;
-  uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][2 KB] accumulator transposes
-  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kXposeWarp);
+  uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][2][2 KB] staging tiles, 1024-B aligned
+  uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kStageWarp);
   uint64_t* a_full = bars;                                  // [kHaloSlots]
   uint64_t* a_empty = a_full + kHaloSlots;
   uint64_t* b_full = a_empty + kHaloSlots;                  // [stages]
@@ -907,6 +917,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     for (int s = 0; s < kHaloSlots; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], kEpiWarps); }
     // a multicast weight stage is refilled only after the consumers of ALL CTAs of the cluster released it
     for (int s = 0; s < stages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], kEpiWarps * CL); }
+    if (d.tma_out) prefetch_tmap(&P.tmOut);
     fence_barrier_init();
   }
   __syncthreads();
@@ -917,16 +928,21 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
   if (warp >= kEpiWarps) {
     if (warp == kTmaWarp) {
       // whole warp in uniform control flow, one elected lane issues the copies
+      GemmTimeline tl;
+      const long long tl_start = tl.now();
       int as = 0; uint32_t aph = 0;
       int bs = 0; uint32_t bph = 0;
       for (int ti = it.first; ti < it.count; ti += it.step) {
         TileCoord c = decode_tile(d, it.tile(ti));
+        tl.tile();
         int kbase = 0;                                       // first 64-wide K block of this source in the weights
         for (int s = 0; s < d.num_src; ++s) {
           const int nch = d.chunks[s];
           for (int ch = 0; ch < nch; ++ch) {
             if (d.rs_h[s] == 0) {                            // (resampled sources: the producer warps own the slot)
+              const long long tl_w = tl.now();
               mbar_wait(&a_empty[as], aph ^ 1);
+              tl.add(1, tl_w);
               if (elect_one()) {
                 mbar_expect_tx(&a_full[as], kHaloBytes);
                 tma_load_4d(smem + as * kHaloSlot, &P.tmA[s], &a_full[as], ch * kBlockK, c.x0 - 1, c.y0 - 1, c.img);
@@ -934,7 +950,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
             }
             if (++as == kHaloSlots) { as = 0; aph ^= 1; }
             for (int tap0 = 0; tap0 < 9; tap0 += kc) {
+              const long long tl_w = tl.now();
               mbar_wait(&b_empty[bs], bph ^ 1);
+              tl.add(1, tl_w);
               if (elect_one()) {
                 mbar_expect_tx(&b_full[bs], b_stage_bytes);
                 if (MC) {
@@ -955,6 +973,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
           kbase += 9 * nch;
         }
       }
+      tl.add(2, tl_start);
+      if (lane == 0) tl.flush(0, 3);
     } else if (warp < kRsWarp0 + 2 && d.rs_any) {
       // ===================== resample producers: halo tiles of the sources read through a bilinear resample =====================
       int as = 0; uint32_t aph = 0;
@@ -979,7 +999,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     }
   } else {
     // ===================== consumers (warps 0..7): wgmma over the nine shifted views of each halo tile + epilogue =====
-    float* buf = reinterpret_cast<float*>(xpose + warp * kXposeWarp);
+    EpiTma et;
+    et.tm = &P.tmOut; et.stg_ptr = xpose + warp * kStageWarp; et.stg = smem_u32(et.stg_ptr); et.cur = 0;
+    float* buf = reinterpret_cast<float*>(et.stg_ptr);
     const int arow = 16 * warp + (lane & 15);               // tile row this lane addresses for ldmatrix
     const uint32_t a_off = static_cast<uint32_t>(((arow >> 3) * kHaloW + (arow & 7)) * 128);
     float acc[BN / 2];
@@ -987,18 +1009,26 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     int as = 0; uint32_t aph = 0;
     int bs = 0; uint32_t bph = 0;
     int rbs = 0;                                            // oldest B stage not yet released
+    GemmTimeline tl;
+    const long long tl_start = tl.now();
     for (int ti = it.first; ti < it.count; ti += it.step) {
       const TileCoord c = decode_tile(d, it.tile(ti));
+      tl.tile();
+      const long long tl_main = tl.now();
       uint32_t accum = 0;
       for (int s = 0; s < d.num_src; ++s) {
         for (int ch = 0; ch < d.chunks[s]; ++ch) {
+          long long tl_w = tl.now();
           mbar_wait(&a_full[as], aph);
+          tl.add(1, tl_w);
           const uint32_t a_base = smem_u32(smem + as * kHaloSlot) + a_off;
           uint32_t sb = 0;
 #pragma unroll
           for (int tap = 0; tap < 9; ++tap) {
             if (tap % kc == 0) {
+              tl_w = tl.now();
               mbar_wait(&b_full[bs], bph);
+              tl.add(1, tl_w);
               sb = smem_u32(smem_b + bs * b_stage_bytes);
               if (++bs == stages) { bs = 0; bph ^= 1; }
             }
@@ -1023,9 +1053,19 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
           if (++as == kHaloSlots) { as = 0; aph ^= 1; }
         }
       }
-      epilogue_tile(d, c, acc, warp, lane, buf, nullptr);
+      tl.add(2, tl_main);
+      const long long tl_epi = tl.now();
+      // plain bf16 outputs (the host sets tma_out for the whole launch): fragment layout, stmatrix staging, bulk
+      // stores of {G ch, 8 px, 2 rows} boxes (TMA clips pixels past W / H, columns past the output and the phantom
+      // img >= NB tile of a cluster); everything else row per thread
+      if (d.tma_out) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64>(d, et, acc, c, warp, lane);
+      else epilogue_tile(d, c, acc, warp, lane, buf, nullptr);
       __syncwarp();
+      tl.add(3, tl_epi);
     }
+    if (lane == 0) bulk_wait0();    // the staging tiles are read (and the writes performed) before the CTA retires
+    tl.add(4, tl_start);
+    if (lane == 0 && (warp & 3) == 0) tl.flush(3, 5);
   }
   __syncthreads();
   if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
@@ -1113,7 +1153,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     const int b_bytes = halo_kc(d.block_n) * d.block_n * kBlockK * 2;     // one weight stage
     const int hstages = halo_stages(d.block_n);
     size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * kHaloSlot + static_cast<size_t>(hstages) * b_bytes +
-                   kEpiWarps * kXposeWarp + kBarBytes;
+                   kEpiWarps * kStageWarp + kBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
       // weight-multicast clusters of cl CTAs over (m-tile group, n-tile) work items.  Every CTA is persistent, so the grid
