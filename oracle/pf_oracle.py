@@ -182,36 +182,27 @@ def exp_attractor(dx, alpha=300.0, gamma=2):
     return torch.exp(-alpha * dx.abs().pow(gamma)) * dx
 
 
-def metric_head(w, x, x_blocks, last, rel_cond, hp, taps=None):
-    """x: bottleneck (B,C,h0,w0); x_blocks: 4 maps low->high; last: (B,32,H,W); rel_cond: (B,1,H,W)."""
-    b_prev = _mlp2(w.sub('seed_bin_regressor.'), x, F.softplus)
-    prev_emb = _mlp2(w.sub('seed_projector.'), x)
-    for i, xb in enumerate(x_blocks):
-        emb = _mlp2(w.sub('projectors.%d.' % i), xb)
-        size = xb.shape[-2:]
-        A = _mlp2(w.sub('attractors.%d.' % i), emb + up(prev_emb, size), F.softplus)
-        b = up(b_prev, size)
-        dist = exp_attractor if _get(hp, 'attractor_type', 'exp') == 'exp' else inv_attractor       # ATT:186-189
-        delta = dist(A.unsqueeze(2) - b.unsqueeze(1))
-        kind = _get(hp, 'attractor_kind', 'sum')
-        delta = delta.mean(dim=1) if kind == 'mean' else delta.sum(dim=1)
-        b_prev, prev_emb = b + delta, emb
-        if taps is not None:
-            taps['b%d' % i] = b_prev
-    b_centers = b_prev
-    size = last.shape[-2:]
-    z = torch.cat([last, up(rel_cond, size), up(prev_emb, size)], dim=1)
-    c = w.sub('conditional_log_binomial.')
-    pt = F.softplus(c.conv('mlp.2', F.gelu(c.conv('mlp.0', z))))
+def attractor_update(A, b_prev, kind='sum', attractor_type='exp'):
+    """One AttractorLayerUnnormed step after its MLP (ATT:179-205): A (B,nA,h,w) attractor points, b_prev
+    (B,nbins,h',w') bin centres up-sampled to (h, w) and shifted by the mean or sum over the attractors."""
+    b = up(b_prev, A.shape[-2:])
+    dist = exp_attractor if attractor_type == 'exp' else inv_attractor                            # ATT:186-189
+    delta = dist(A.unsqueeze(2) - b.unsqueeze(1))
+    delta = delta.mean(dim=1) if kind == 'mean' else delta.sum(dim=1)
+    return b + delta
+
+
+def log_binomial_depth(pt, b_centers, min_t, max_t):
+    """ConditionalLogBinomial after its MLP (DIS:110-121, LogBinomial DIS:51-69) and the expectation over the bin
+    centres up-sampled to pt's size (ZD:214-219): pt (B,4,H,W) softplus outputs, b_centers (B,K,h,w) -> (B,1,H,W)."""
     p, t = pt[:, :2] + 1e-4, pt[:, 2:] + 1e-4
     p = p[:, 0] / (p[:, 0] + p[:, 1])
     t = (t[:, 0] / (t[:, 0] + t[:, 1])).unsqueeze(1)
-    min_t, max_t = _get(hp, 'min_temp'), _get(hp, 'max_temp')
     t = (max_t - min_t) * t + min_t
     # LogBinomial (DIS:51-69), Stirling form of log C(K-1, k)
-    K = _get(hp, 'n_bins', 64)
-    k = torch.arange(K, dtype=torch.float32, device=x.device).view(1, K, 1, 1)
-    n_ = torch.tensor(float(K - 1), device=x.device) + 1e-7
+    K = b_centers.shape[1]
+    k = torch.arange(K, dtype=torch.float32, device=pt.device).view(1, K, 1, 1)
+    n_ = torch.tensor(float(K - 1), device=pt.device) + 1e-7
     k_ = k + 1e-7
     logc = n_ * torch.log(n_) - k_ * torch.log(k_) - (n_ - k_) * torch.log(n_ - k_ + 1e-7)
     p = p.unsqueeze(1)
@@ -219,7 +210,25 @@ def metric_head(w, x, x_blocks, last, rel_cond, hp, taps=None):
     p = torch.clamp(p, 1e-4, 1)
     y = logc + k * torch.log(p) + (K - 1 - k) * torch.log(q)
     prob = torch.softmax(y / t, dim=1)
-    return torch.sum(prob * up(b_centers, size), dim=1, keepdim=True)
+    return torch.sum(prob * up(b_centers, pt.shape[-2:]), dim=1, keepdim=True)
+
+
+def metric_head(w, x, x_blocks, last, rel_cond, hp, taps=None):
+    """x: bottleneck (B,C,h0,w0); x_blocks: 4 maps low->high; last: (B,32,H,W); rel_cond: (B,1,H,W)."""
+    b_prev = _mlp2(w.sub('seed_bin_regressor.'), x, F.softplus)
+    prev_emb = _mlp2(w.sub('seed_projector.'), x)
+    for i, xb in enumerate(x_blocks):
+        emb = _mlp2(w.sub('projectors.%d.' % i), xb)
+        A = _mlp2(w.sub('attractors.%d.' % i), emb + up(prev_emb, xb.shape[-2:]), F.softplus)
+        b_prev = attractor_update(A, b_prev, _get(hp, 'attractor_kind', 'sum'), _get(hp, 'attractor_type', 'exp'))
+        prev_emb = emb
+        if taps is not None:
+            taps['b%d' % i] = b_prev
+    size = last.shape[-2:]
+    z = torch.cat([last, up(rel_cond, size), up(prev_emb, size)], dim=1)
+    c = w.sub('conditional_log_binomial.')
+    pt = F.softplus(c.conv('mlp.2', F.gelu(c.conv('mlp.0', z))))
+    return log_binomial_depth(pt, b_prev, _get(hp, 'min_temp'), _get(hp, 'max_temp'))
 
 
 # --------------------------------------------------------------------------------------------------------------
