@@ -1,5 +1,6 @@
-"""Minimal `MODELS` registry with the reference's call surface (`estimator/registry/registry.py:7`,
-`estimator/models/builder.py:6-8`): `MODELS.build(dict(type='PatchFusion', config=...))`."""
+"""Minimal `MODELS` / `DATASETS` registries with the reference's call surface (`estimator/registry/registry.py:7-8`,
+`estimator/models/builder.py:6-8`, `estimator/datasets/builder.py:5-7`):
+`MODELS.build(dict(type='PatchFusion', config=...))`, `DATASETS.build(dict(type='UnrealStereo4kDataset', ...))`."""
 
 
 class _Registry:
@@ -19,8 +20,9 @@ class _Registry:
         cfg = dict(cfg)
         typ = cfg.pop('type')
         if typ not in self._mods:
-            raise KeyError('%s is not in the %s registry (only the hot-path model is built)' % (typ, self.name))
+            raise KeyError('%s is not in the %s registry (registered: %s)' % (typ, self.name, ', '.join(sorted(self._mods))))
         return self._mods[typ](**cfg)
 
 
 MODELS = _Registry('model')
+DATASETS = _Registry('dataset')

@@ -202,6 +202,23 @@ int pf_ingest_u8(const uint8_t* img_hwc, int32_t H, int32_t W, int32_t bgr, int3
  * (depth * scale) cast (estimator/tester/tester.py:75-76, scale 256). */
 int pf_depth_to_u16(const float* depth, int32_t H, int32_t W, int32_t OH, int32_t OW, float scale, uint16_t* out,
                     void* stream);
+/* U4K raw frame: uint8 HWC (bgr != 0: stored BGR) -> planar RGB fp32 u8 / 255 at the same size, correctly rounded,
+ * no resample (estimator/datasets/u4k_dataset.py:115-129). */
+int pf_ingest_raw_u8(const uint8_t* img_hwc, int32_t H, int32_t W, int32_t bgr, float* out_planar, void* stream);
+/* Evaluation ground truth in one pass over a source map [H, W]: depth [H, W] fp32 and boundary [H, W] uint8, where a
+ * pixel is an edge when |e[p] - e[q]| > th for a 4-neighbour q (get_boundaries(e, th, dilation=0),
+ * estimator/utils/image_ops.py:25-31; a NaN difference is no edge).  kind (PF_GT_*) picks the dataset branch:
+ *   U4K        src fp32 disparity; e = src; depth = factor / src
+ *   MID        src fp32 disparity; e = src with +inf -> 0; depth = factor / (src + doffs) / 1000, +inf src -> 0
+ *   ETH3D      src fp32 depth; depth = e = nan_to_num(src, nan=0, posinf=0, neginf=0)
+ *   CITYSCAPES src uint16 disparity x; x > 0 -> (x - 1) / 256; depth = e = nan_to_num(factor / x)
+ * factor and doffs are the float32 roundings of the reference's Python floats; all arithmetic is IEEE fp32. */
+#define PF_GT_U4K 0
+#define PF_GT_MID 1
+#define PF_GT_ETH3D 2
+#define PF_GT_CITYSCAPES 3
+int pf_gt_prepare(const void* src, int32_t kind, int32_t H, int32_t W, float factor, float doffs, float th,
+                  float* depth, uint8_t* boundary, void* stream);
 
 /* compute_metrics / compute_errors / soft_edge_error (estimator/utils/metric.py:10-50, 67-72, 97-148) as one fused
  * reduction over the ground-truth grid.  pred [PH,PW] fp32 is resampled (bilinear, align_corners=False, metric.py:101-104)

@@ -23,6 +23,38 @@ def ingest(image_u8, image_raw_shape, device, bgr=True):
     return out
 
 
+def ingest_raw(image_u8, bgr=True):
+    """image_u8: HxWx3 uint8 tensor on the GPU (a U4K raw frame, stored BGR).  Returns image_hr (1,3,H,W) fp32 RGB,
+    u8 / 255 correctly rounded at the same size (`u4k_dataset.py:126-129`; no resample)."""
+    assert image_u8.is_cuda and image_u8.dtype == torch.uint8 and image_u8.dim() == 3 and image_u8.shape[2] == 3
+    src = image_u8.contiguous()
+    H, W = src.shape[:2]
+    out = torch.empty((1, 3, H, W), dtype=torch.float32, device=src.device)
+    ops.call('pf_ingest_raw_u8', src, H, W, 1 if bgr else 0, out, ops.stream_ptr())
+    return out
+
+
+GT_KINDS = {'u4k': 0, 'mid': 1, 'eth3d': 2, 'cityscapes': 3}
+GT_SOURCE_DTYPES = {'u4k': torch.float32, 'mid': torch.float32, 'eth3d': torch.float32, 'cityscapes': torch.uint16}
+
+
+def gt_prepare(src, kind, factor=0.0, doffs=0.0, th=1.0):
+    """Ground truth of one evaluation image on the GPU (pf_gt_prepare): src [H,W] on the device (fp32; uint16 for
+    'cityscapes') -> (depth_gt (1,1,H,W) fp32, boundary (1,1,H,W) uint8), bit-identical to the reference's numpy
+    branch of that dataset.  factor / doffs are the reference's Python floats; they are rounded to float32 here, as
+    numpy 2 does when it combines them with a float32 array."""
+    if kind not in GT_KINDS:
+        raise NotImplementedError('ground truth of kind %r' % (kind,))
+    assert src.is_cuda and src.dim() == 2 and src.dtype == GT_SOURCE_DTYPES[kind], (src.dtype, kind)
+    src = src.contiguous()
+    H, W = src.shape
+    depth = torch.empty((1, 1, H, W), dtype=torch.float32, device=src.device)
+    boundary = torch.empty((1, 1, H, W), dtype=torch.uint8, device=src.device)
+    ops.call('pf_gt_prepare', src, GT_KINDS[kind], H, W, C.c_float(factor), C.c_float(doffs), C.c_float(th), depth,
+             boundary, ops.stream_ptr())
+    return depth, boundary
+
+
 def depth_to_u16(depth, size=None, scale=256.0):
     """depth (1,1,h,w) or (h,w) fp32 on the GPU -> uint16 tensor (H,W): nearest resize to `size` then *scale."""
     d = depth.reshape(depth.shape[-2:]).float().contiguous()

@@ -76,6 +76,8 @@ SIGNATURES = {
     'pf_f32_to_bf16': [_p, _ll, _p, _p],
     'pf_ingest_u8': [_p, _i, _i, _i, _i, _i, _p, _p],
     'pf_depth_to_u16': [_p, _i, _i, _i, _i, _f, _p, _p],
+    'pf_ingest_raw_u8': [_p, _i, _i, _i, _p, _p],
+    'pf_gt_prepare': [_p, _i, _i, _i, _f, _f, _f, _p, _p, _p],
     'pf_depth_metrics': [_p, _i, _i, _p, _i, _i, _f, _f, _p, _p, _p, _i, _p, _p],
     'pf_colorize_u8': [_p, _ll, _f, _f, _f, _p, _i, _p, _p],
     'pf_g2l_embed': [_p, _i, _p, _i, _i, _p, _p],
