@@ -324,10 +324,26 @@ def shift_mask(Hp, Wp, ws, device):
     return torch.where(m != 0, torch.full_like(m, -100.0), torch.zeros_like(m))
 
 
+def window_attention(qkv, table, index, heads, mask=None):
+    """SW:139-161 without the projections: qkv (nW, N, 3C) of the windowed tokens, the (2ws-1)^2 x heads bias table,
+    the (N, N) relative position index and the (nW, N, N) shift mask (None: no shift) -> (nW, N, C)."""
+    nW, N, C3 = qkv.shape
+    C = C3 // 3
+    hd = C // heads
+    qkv = qkv.reshape(nW, N, 3, heads, hd).permute(2, 0, 3, 1, 4)
+    q, k, v = qkv[0] * hd ** -0.5, qkv[1], qkv[2]
+    a = q @ k.transpose(-2, -1)
+    bias = table[index.reshape(-1)]
+    a = a + bias.view(N, N, heads).permute(2, 0, 1).unsqueeze(0)
+    if mask is not None:
+        a = a + mask.unsqueeze(1)
+    a = a.softmax(dim=-1)
+    return (a @ v).transpose(1, 2).reshape(nW, N, C)
+
+
 def swin_block(w, x, H, W, heads, shift, mask):
     B, L, C = x.shape
     ws = WINDOW
-    hd = C // heads
     h = w.ln('norm1', x, 1e-5).view(B, H, W, C)
     pb, pr = (ws - H % ws) % ws, (ws - W % ws) % ws
     h = F.pad(h, (0, 0, 0, pr, 0, pb))
@@ -335,16 +351,8 @@ def swin_block(w, x, H, W, heads, shift, mask):
     if shift:
         h = torch.roll(h, shifts=(-shift, -shift), dims=(1, 2))
     win = _windows(h, ws)
-    nW, N = win.shape[0], ws * ws
-    qkv = w.linear('attn.qkv', win).reshape(nW, N, 3, heads, hd).permute(2, 0, 3, 1, 4)
-    q, k, v = qkv[0] * hd ** -0.5, qkv[1], qkv[2]
-    a = q @ k.transpose(-2, -1)
-    bias = w('attn.relative_position_bias_table')[w('attn.relative_position_index').view(-1)]
-    a = a + bias.view(N, N, heads).permute(2, 0, 1).unsqueeze(0)
-    if shift:
-        a = a + mask.unsqueeze(1)
-    a = a.softmax(dim=-1)
-    o = (a @ v).transpose(1, 2).reshape(nW, N, C)
+    o = window_attention(w.linear('attn.qkv', win), w('attn.relative_position_bias_table'),
+                         w('attn.relative_position_index'), heads, mask if shift else None)
     o = w.linear('attn.proj', o)
     o = _unwindows(o, ws, Hp, Wp)
     if shift:
