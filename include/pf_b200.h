@@ -273,6 +273,20 @@ int pf_add_upsampled(const void* a, int32_t B, int32_t H, int32_t W, int32_t C, 
 #define PF_ATTRACTOR_EXP 2
 int pf_attractor(const float* A, int32_t A_ld, int32_t nA, const float* b_prev, int32_t PH, int32_t PW, int32_t B, int32_t H,
                  int32_t W, int32_t nbins, int32_t flags, float* b_out, void* stream);
+/* AttractorLayer (attractor.py:100-135, the normed and hybrid2 heads): as pf_attractor with the attractor points
+ * A + 1e-3, A holding the even `_net` channels only (attractor.py:105-106).  b_out receives the normalised, unsorted
+ * b_new; centers (nullable; the last level) clip(sort((max - min) b_new + min), min, max) per pixel. */
+int pf_attractor_normed(const float* A, int32_t A_ld, int32_t nA, const float* b_prev, int32_t PH, int32_t PW, int32_t B,
+                        int32_t H, int32_t W, int32_t nbins, int32_t flags, float min_depth, float max_depth, float* b_out,
+                        float* centers, void* stream);
+/* seed bin centres from the seed regressor's `_net` output S [pixels, S_ld] (fp32; ReLU'd for PF_SEED_NORMED, else
+ * softplus'd) into out [pixels, nbins].  PF_SEED_NORMED: SeedBinRegressor (localbins_layers.py:51-67): widths
+ * (max - min) (S + 1e-3) / sum, centres the midpoints of min + cumsum(widths); else the centres are S.
+ * PF_SEED_TO_UNIT: then (c - min) / (max - min) (zoedepth_v1.py:176-181). */
+#define PF_SEED_NORMED 1
+#define PF_SEED_TO_UNIT 2
+int pf_seed_bins(const float* S, int32_t S_ld, int64_t pixels, int32_t nbins, int32_t flags, float min_depth,
+                 float max_depth, float* out, void* stream);
 /* depth = sum_k softmax_k(logbinom(p)/t) * up(b_centers)_k from the 4-channel softplus'd pt map */
 int pf_logbinom_depth(const float* pt, int32_t pt_ld, const float* b_centers, int32_t BH, int32_t BW, int32_t B, int32_t H, int32_t W,
                       int32_t nbins, float min_temp, float max_temp, float* depth, void* stream);
@@ -347,7 +361,13 @@ typedef struct pf_head {                  /* metric-bins head: zoedepth_v1.py:17
   int32_t attractor_flags;                /* PF_ATTRACTOR_MEAN | PF_ATTRACTOR_EXP */
   int32_t has_rel;                        /* CLB input carries the relative-depth channel (branch heads) */
   float min_temp, max_temp;
+  int32_t bin_centers_type;               /* PF_BINS_*: seed regressor and attractor form (zoedepth_v1.py:90-105) */
+  float min_depth, max_depth;             /* the head's depth range (branch config; top-level for the fusion head) */
 } pf_head;
+#define PF_BINS_SOFTPLUS 0                /* SeedBinRegressorUnnormed + AttractorLayerUnnormed */
+#define PF_BINS_NORMED 1                  /* SeedBinRegressor + AttractorLayer */
+#define PF_BINS_HYBRID1 2                 /* SeedBinRegressor + AttractorLayerUnnormed */
+#define PF_BINS_HYBRID2 3                 /* SeedBinRegressorUnnormed + AttractorLayer */
 
 typedef struct pf_branch {                /* one ZoeDepth(Depth-Anything) branch */
   int32_t H, W;                           /* patch_process_shape (multiples of 14) */

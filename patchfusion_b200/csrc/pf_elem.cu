@@ -693,9 +693,14 @@ __global__ void add_upsampled_kernel(const bf16* __restrict__ a, int B, int H, i
 
 // one warp per pixel (grid-stride), 2 bins per lane (nbins == 64): b = up(b_prev); b += mean_a|sum_a( dist(dx) ),
 // dx = A_a - b, dist = inverse (dx / (1 + 300 dx^2)) or exponential (exp(-300 dx^2) dx) attractor.  The <= 16 attractor points of the pixel are read once per warp.
-__global__ void attractor_kernel(const float* __restrict__ A, int A_ld, int nA, const float* __restrict__ b_prev, int PH,
-                                 int PW, int B, int H, int W, int nbins, int kind_mean, int type_exp, float sy, float sx,
-                                 float* __restrict__ b_out) {
+// NORMED (AttractorLayer, attractor.py:100-135): the attractor points are A + 1e-3 (A holds the even `_net` channels
+// only: A_normed is overwritten by A[:, :, 0], attractor.py:105-106), and `centers`, when given, receives
+// clip(sort((max - min) b + min), min, max), sorted per pixel by a bitonic network over the warp's 64 values.
+template <bool NORMED>
+__device__ __forceinline__ void attractor_body(const float* __restrict__ A, int A_ld, int nA, const float* __restrict__ b_prev,
+                                               int PH, int PW, int B, int H, int W, int nbins, int kind_mean, int type_exp,
+                                               float sy, float sx, float* __restrict__ b_out, float min_d, float max_d,
+                                               float* __restrict__ centers) {
   const int lane = threadIdx.x & 31;
   const int warps = (gridDim.x * blockDim.x) >> 5;
   const int total = B * H * W, hw = H * W;
@@ -710,7 +715,8 @@ __global__ void attractor_kernel(const float* __restrict__ A, int A_ld, int nA, 
     const float* r01 = base + (static_cast<size_t>(y0) * PW + x1) * nbins;
     const float* r10 = base + (static_cast<size_t>(y1) * PW + x0) * nbins;
     const float* r11 = base + (static_cast<size_t>(y1) * PW + x1) * nbins;
-    const float av = lane < nA ? __ldg(A + static_cast<size_t>(p) * A_ld + lane) : 0.f;
+    float av = lane < nA ? __ldg(A + static_cast<size_t>(p) * A_ld + lane) : 0.f;
+    if (NORMED) av += 1e-3f;
     float bc[2], s[2] = {0.f, 0.f};
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -728,10 +734,109 @@ __global__ void attractor_kernel(const float* __restrict__ A, int A_ld, int nA, 
         s[i] += type_exp ? __expf(-300.f * dx * dx) * dx : dx / (1.f + 300.f * dx * dx);
       }
     }
+    float v[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       if (kind_mean) s[i] /= nA;
-      b_out[static_cast<size_t>(p) * nbins + lane + 32 * i] = bc[i] + s[i];
+      v[i] = bc[i] + s[i];
+      b_out[static_cast<size_t>(p) * nbins + lane + 32 * i] = v[i];
+    }
+    if (NORMED && centers != nullptr) {
+      const float range = max_d - min_d;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) v[i] = range * v[i] + min_d;
+      // bitonic sort of the 64 values, element k = lane + 32 i: every (size, stride) step pairs k with k ^ stride and
+      // keeps the smaller value at the lower index where (k & size) == 0 (ascending run), the larger elsewhere.  The
+      // stride-32 partner is the lane's other register; the others live in lane ^ stride.
+#pragma unroll
+      for (int size = 2; size <= 64; size <<= 1) {
+#pragma unroll
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+          if (stride == 32) {
+            const float lo = fminf(v[0], v[1]), hi = fmaxf(v[0], v[1]);
+            v[0] = lo; v[1] = hi;
+          } else {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int k = lane + 32 * i;
+              const float o = __shfl_xor_sync(0xffffffffu, v[i], stride);
+              const bool up = (k & size) == 0, lower = (k & stride) == 0;
+              v[i] = (up == lower) ? fminf(v[i], o) : fmaxf(v[i], o);
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+        centers[static_cast<size_t>(p) * nbins + lane + 32 * i] = fminf(fmaxf(v[i], min_d), max_d);
+    }
+  }
+}
+
+__global__ void attractor_kernel(const float* __restrict__ A, int A_ld, int nA, const float* __restrict__ b_prev, int PH,
+                                 int PW, int B, int H, int W, int nbins, int kind_mean, int type_exp, float sy, float sx,
+                                 float* __restrict__ b_out) {
+  attractor_body<false>(A, A_ld, nA, b_prev, PH, PW, B, H, W, nbins, kind_mean, type_exp, sy, sx, b_out, 0.f, 0.f, nullptr);
+}
+
+__global__ void attractor_normed_kernel(const float* __restrict__ A, int A_ld, int nA, const float* __restrict__ b_prev,
+                                        int PH, int PW, int B, int H, int W, int nbins, int kind_mean, int type_exp,
+                                        float sy, float sx, float* __restrict__ b_out, float min_d, float max_d,
+                                        float* __restrict__ centers) {
+  attractor_body<true>(A, A_ld, nA, b_prev, PH, PW, B, H, W, nbins, kind_mean, type_exp, sy, sx, b_out, min_d, max_d,
+                       centers);
+}
+
+// SeedBinRegressor's centres (localbins_layers.py:51-67) from its `_net` output S (ReLU'd), one warp per pixel
+// (grid-stride), 2 bins per lane (nbins == 64): w_k = (max - min) (S_k + 1e-3) / sum_j (S_j + 1e-3), edges = min +
+// cumsum(w) (the min_depth pad in front), c_k = (edge_k + edge_k+1) / 2.  The sum is a butterfly; the cumsum a
+// Hillis-Steele scan of each 32-bin half, the upper half offset by the lower half's total.  PF_SEED_NORMED off: the
+// centres are S itself (SeedBinRegressorUnnormed).  PF_SEED_TO_UNIT: (c - min) / (max - min), the b_prev of the
+// normed attractors (zoedepth_v1.py:176-181).
+__global__ void seed_bins_kernel(const float* __restrict__ S, int S_ld, long long total, int normed, int to_unit,
+                                 float min_d, float max_d, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  const float range = max_d - min_d;
+  for (long long p = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; p < total; p += warps) {
+    float c[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) c[i] = __ldg(S + p * S_ld + lane + 32 * i);
+    if (normed) {
+      float w[2], sum;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) w[i] = c[i] + 1e-3f;
+      sum = w[0] + w[1];
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      float inc[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        w[i] = range * (w[i] / sum);
+        inc[i] = w[i];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const float t = __shfl_up_sync(0xffffffffu, inc[i], o);
+          if (lane >= o) inc[i] += t;
+        }
+      }
+      // exclusive prefix = the left neighbour's inclusive one, so bin k's upper edge is bin k+1's lower edge bit for bit
+      float exc[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        exc[i] = __shfl_up_sync(0xffffffffu, inc[i], 1);
+        if (lane == 0) exc[i] = 0.f;
+      }
+      const float half = __shfl_sync(0xffffffffu, inc[0], 31);
+      exc[1] = lane == 0 ? half : exc[1] + half;
+      inc[1] += half;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) c[i] = 0.5f * ((min_d + exc[i]) + (min_d + inc[i]));
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      if (to_unit) c[i] = (c[i] - min_d) / range;
+      out[p * 64 + lane + 32 * i] = c[i];
     }
   }
 }
@@ -1145,6 +1250,35 @@ int pf_attractor(const float* A, int32_t A_ld, int32_t nA, const float* b_prev, 
   attractor_kernel<<<blocks, 256, 0, ST>>>(A, A_ld, nA, b_prev, PH, PW, B, H, W, nbins, kind_mean, type_exp,
                                            ac_scale(PH, H), ac_scale(PW, W), b_out);
   return check_launch("attractor_kernel");
+}
+
+int pf_attractor_normed(const float* A, int32_t A_ld, int32_t nA, const float* b_prev, int32_t PH, int32_t PW, int32_t B,
+                        int32_t H, int32_t W, int32_t nbins, int32_t flags, float min_depth, float max_depth, float* b_out,
+                        float* centers, void* stream) {
+  if (nbins != 64 || nA > 32) return set_error("pf_attractor_normed: n_bins must be 64 and n_attractors <= 32");
+  if (flags & ~3) return set_error("pf_attractor_normed: unknown flags %d", flags);
+  if (!(max_depth > min_depth)) return set_error("pf_attractor_normed: max_depth must exceed min_depth");
+  const int kind_mean = flags & PF_ATTRACTOR_MEAN, type_exp = (flags & PF_ATTRACTOR_EXP) ? 1 : 0;
+  long long warps_needed = static_cast<long long>(B) * H * W;
+  const long long cap = 8LL * sm_count();
+  unsigned blocks = static_cast<unsigned>(warps_needed < cap * 8 ? (warps_needed + 7) / 8 : cap);
+  attractor_normed_kernel<<<blocks, 256, 0, ST>>>(A, A_ld, nA, b_prev, PH, PW, B, H, W, nbins, kind_mean, type_exp,
+                                                  ac_scale(PH, H), ac_scale(PW, W), b_out, min_depth, max_depth, centers);
+  return check_launch("attractor_normed_kernel");
+}
+
+int pf_seed_bins(const float* S, int32_t S_ld, int64_t pixels, int32_t nbins, int32_t flags, float min_depth,
+                 float max_depth, float* out, void* stream) {
+  if (nbins != 64) return set_error("pf_seed_bins: n_bins must be 64");
+  if (flags & ~3) return set_error("pf_seed_bins: unknown flags %d", flags);
+  if (S_ld < 64) return set_error("pf_seed_bins: S_ld must be >= 64");
+  if (!(max_depth > min_depth)) return set_error("pf_seed_bins: max_depth must exceed min_depth");
+  const long long cap = 8LL * sm_count();
+  unsigned blocks = static_cast<unsigned>(pixels < cap * 8 ? (pixels + 7) / 8 : cap);
+  if (blocks == 0) return 0;
+  seed_bins_kernel<<<blocks, 256, 0, ST>>>(S, S_ld, pixels, flags & PF_SEED_NORMED, (flags & PF_SEED_TO_UNIT) ? 1 : 0,
+                                           min_depth, max_depth, out);
+  return check_launch("seed_bins_kernel");
 }
 
 int pf_logbinom_depth(const float* pt, int32_t pt_ld, const float* b_centers, int32_t BH, int32_t BW, int32_t B,

@@ -192,23 +192,56 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
     }
     return o;
   };
-  MapF b_prev = mlp_f32(Hd.seed0, Hd.seed2, x, PF_ACT_SOFTPLUS);        // seed bin centres, fp32 [B,h,w,64]
-  Map prev_emb = mlp_bf16(Hd.seedproj0, Hd.seedproj2, x);
+  // bin_centers_type (zoedepth_v1.py:90-105): SeedBinRegressor ends in ReLU and normalises widths into centres,
+  // AttractorLayer ends in ReLU and sorts and clips its metric output.  The softplus head launches and allocates exactly
+  // as if the type did not exist: the extra buffers below come only with the other types.
+  const int type = Hd.bin_centers_type;
+  if (type < PF_BINS_SOFTPLUS || type > PF_BINS_HYBRID2) {
+    c.chk(set_error("metric head: unknown bin_centers_type %d", type));
+    return;
+  }
+  const bool normed_seed = type == PF_BINS_NORMED || type == PF_BINS_HYBRID1;
+  const bool normed_att = type == PF_BINS_NORMED || type == PF_BINS_HYBRID2;
+  MapF b_prev = mlp_f32(Hd.seed0, Hd.seed2, x, normed_seed ? PF_ACT_RELU : PF_ACT_SOFTPLUS);   // fp32 [B,h,w,64]
   const float* b_t = b_prev.p;
+  if (type != PF_BINS_SOFTPLUS) {     // seed centres; normalised to [0, 1] for the normed attractors (zoedepth_v1.py:176-181)
+    const long long px = static_cast<long long>(B) * x.H * x.W;
+    float* sb = static_cast<float*>(c.alloc(static_cast<size_t>(px) * nb * 4));
+    if (c.live())
+      c.chk(pf_seed_bins(b_prev.p, b_prev.ld, px, nb, (normed_seed ? PF_SEED_NORMED : 0) | (normed_att ? PF_SEED_TO_UNIT : 0),
+                         Hd.min_depth, Hd.max_depth, sb, c.stream));
+    b_t = sb;
+    c.tap_out("seed", sb, 1, px, nb, nb);
+  }
+  Map prev_emb = mlp_bf16(Hd.seedproj0, Hd.seedproj2, x);
+  const float* centers = nullptr;
   int ph = x.H, pw = x.W;
   for (int i = 0; i < 4; ++i) {
     const Map& xb = x_blocks[i];
     Map emb = mlp_bf16(Hd.proj0[i], Hd.proj2[i], xb);
     Map s = c.map(B, xb.H, xb.W, E);
     if (c.live()) c.chk(pf_add_upsampled(emb.p, B, xb.H, xb.W, E, prev_emb.p, prev_emb.H, prev_emb.W, s.p, c.stream));
-    MapF A = mlp_f32(Hd.att0[i], Hd.att2[i], s, PF_ACT_SOFTPLUS);
-    float* b_new = static_cast<float*>(c.alloc(static_cast<size_t>(B) * xb.H * xb.W * nb * 4));
-    if (c.live())
+    MapF A = mlp_f32(Hd.att0[i], Hd.att2[i], s, normed_att ? PF_ACT_RELU : PF_ACT_SOFTPLUS);
+    const size_t bytes = static_cast<size_t>(B) * xb.H * xb.W * nb * 4;
+    float* b_new = static_cast<float*>(c.alloc(bytes));
+    if (normed_att) {
+      // only the last level's sorted metric centres are read (zoedepth_v1.py:217-219)
+      float* cen = i == 3 ? static_cast<float*>(c.alloc(bytes)) : nullptr;
+      if (c.live())
+        c.chk(pf_attractor_normed(A.p, A.ld, Hd.n_attractors[i], b_t, ph, pw, B, xb.H, xb.W, nb, Hd.attractor_flags,
+                                  Hd.min_depth, Hd.max_depth, b_new, cen, c.stream));
+      if (cen != nullptr) centers = cen;
+    } else if (c.live()) {
       c.chk(pf_attractor(A.p, A.ld, Hd.n_attractors[i], b_t, ph, pw, B, xb.H, xb.W, nb, Hd.attractor_flags, b_new, c.stream));
+    }
     b_t = b_new; ph = xb.H; pw = xb.W; prev_emb = emb;
     char nm[8];
     snprintf(nm, sizeof(nm), "b%d", i);
     c.tap_out(nm, b_new, 1, static_cast<long long>(B) * xb.H * xb.W, nb, nb);
+  }
+  if (normed_att) {
+    c.tap_out("centers", centers, 1, static_cast<long long>(B) * ph * pw, nb, nb);
+    b_t = centers;
   }
   const int H = last.H, W = last.W;
   Map emb_up = resize(c, prev_emb, H, W);

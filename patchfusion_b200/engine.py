@@ -21,9 +21,9 @@ import math
 import torch
 import torch.nn.functional as F
 
-from . import ops
+from . import lib, ops
 from .ops import ACT_GELU, ACT_NONE, ACT_RELU, ACT_SOFTPLUS, call, pad_to, stream_ptr
-from .params import WINDOW, branch_hparams, guided_fusion_hparams, _get
+from .params import WINDOW, branch_hparams, guided_fusion_hparams, normed_attractors, _get
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -107,11 +107,13 @@ class Engine:
         for n in ['seed_bin_regressor', 'seed_projector'] + ['projectors.%d' % i for i in range(4)] + \
                  ['attractors.%d' % i for i in range(4)]:
             Wd[n + '.0'] = self._conv(pre + n + '._net.0')
-            Wd[n + '.2'] = self._conv(pre + n + '._net.2')
-            w2 = self._w(pre + n + '._net.2.weight')
+            w2, b2 = self._w(pre + n + '._net.2.weight'), self._w(pre + n + '._net.2.bias')
+            if n.startswith('attractors') and normed_attractors(hp['bin_centers_type']):
+                # AttractorLayer reads only the even channels of its 2 nA outputs (attractor.py:104-106)
+                w2, b2 = w2[0::2].contiguous(), b2[0::2].contiguous()
+            Wd[n + '.2'] = ops.pack_weight(w2, b2)
             if w2.shape[0] <= 16:       # narrow second layer: fused into the first layer's epilogue (fp32 weights)
-                Wd[n + '.tail'] = (w2.reshape(w2.shape[0], -1).float().contiguous(),
-                                   self._f32(pre + n + '._net.2.bias'))
+                Wd[n + '.tail'] = (w2.reshape(w2.shape[0], -1).float().contiguous(), b2.float().contiguous())
         w0 = self._w(pre + 'conditional_log_binomial.mlp.0.weight')
         b0 = self._w(pre + 'conditional_log_binomial.mlp.0.bias')
         E = hp['bin_embedding_dim']
@@ -232,7 +234,9 @@ class Engine:
         torch.cuda.synchronize(self.dev)
 
     # ------------------------------------------------------------------ C structs for the stage-level ABI
-    def _c_head(self, Wh, hp, bcfg, has_rel):
+    def _c_head(self, Wh, hp, bcfg, has_rel, depth_cfg):
+        """depth_cfg: where the head's min_depth / max_depth come from: the branch config for a branch head, the
+        top-level config for the fusion head (patchfusion.py:149-164)."""
         from . import stage
         H = stage.PfHead()
 
@@ -250,6 +254,9 @@ class Engine:
         H.attractor_flags = (1 if hp['attractor_kind'] == 'mean' else 0) | (2 if hp['attractor_type'] == 'exp' else 0)
         H.has_rel = 1 if has_rel else 0
         H.min_temp, H.max_temp = float(_get(bcfg, 'min_temp')), float(_get(bcfg, 'max_temp'))
+        H.bin_centers_type = lib.BINS_TYPES[hp['bin_centers_type']]
+        # ZoeDepth's constructor defaults (zoedepth_v1.py:40)
+        H.min_depth, H.max_depth = float(_get(depth_cfg, 'min_depth', 1e-3)), float(_get(depth_cfg, 'max_depth', 10))
         return H
 
     def _c_branch(self, which):
@@ -283,7 +290,7 @@ class Engine:
         B.oc1 = stage.layer(Wd['oc1'])
         B.oc2 = stage.layer(Wd['oc2.0'], Wd['oc2.tail'])
         B.conv2 = stage.layer(Wd['conv2'])
-        B.head = self._c_head(Wd['head'], hp, self.bcfg[which], True)
+        B.head = self._c_head(Wd['head'], hp, self.bcfg[which], True, self.bcfg[which])
         return B
 
     def _c_fusion(self):
@@ -310,7 +317,7 @@ class Engine:
                     setattr(blocks[b], k, stage.layer(bw[k]))
             self._keep.append(blocks)
             g.blocks = blocks
-        F_.head = self._c_head(Wf['head'], self.hp['coarse'], self.bcfg['coarse'], False)
+        F_.head = self._c_head(Wf['head'], self.hp['coarse'], self.bcfg['coarse'], False, self.cfg)
         return F_
 
     # ------------------------------------------------------------------ workspaces (one arena per stage role)
@@ -366,6 +373,9 @@ class Engine:
             for k_ in list(taps):
                 if k_[0] == 'b' and k_[1:].isdigit():
                     m = feats[1 + int(k_[1:])]
+                    taps[k_] = taps[k_].view(B, m.hw[0], m.hw[1], -1)
+                elif k_ in ('seed', 'centers'):         # x_d0's grid / the last attractor's (feats[4] = r1)
+                    m = feats[0 if k_ == 'seed' else 4]
                     taps[k_] = taps[k_].view(B, m.hw[0], m.hw[1], -1)
         return depth, feats
 

@@ -13,6 +13,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, os.environ.get('PF_B200_LIBNAME', 'libpf_b200.so'))
 
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SOFTPLUS = 0, 1, 2, 3
+# include/pf_b200.h PF_BINS_* (pf_head.bin_centers_type) and PF_SEED_* (pf_seed_bins flags)
+BINS_TYPES = {'softplus': 0, 'normed': 1, 'hybrid1': 2, 'hybrid2': 3}
+SEED_NORMED, SEED_TO_UNIT = 1, 2
 OPT_TMA_EPILOGUE, OPT_HALO_MULTICAST, OPT_GEMM_MULTICAST, OPT_FUSED_RESAMPLE, OPT_PDL, OPT_RESIZE_SEPARABLE = 0, 1, 2, 3, 4, 5
 
 
@@ -90,6 +93,8 @@ SIGNATURES = {
     'pf_swin_residual_crop_batched': [_p, _p, _i, _i, _i, _i, _i, _i, _p],
     'pf_add_upsampled': [_p, _i, _i, _i, _i, _p, _i, _i, _p, _p],
     'pf_attractor': [_p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p, _p],
+    'pf_attractor_normed': [_p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, _f, _f, _p, _p, _p],
+    'pf_seed_bins': [_p, _i, _ll, _i, _i, _f, _f, _p, _p],
     'pf_logbinom_depth': [_p, _i, _p, _i, _i, _i, _i, _i, _i, _f, _f, _p, _p],
     'pf_stitch_accumulate': [_p, _p, _i, _i, _p, _i, _i, _i, _p, _p, _i, _i, _p],
     'pf_stitch_gather': [_p, _p, _i, _i, _i, _p, _i, _i, _p, _p, _i, _i, _p, _p, _p, _p],

@@ -211,3 +211,19 @@ def crop_resize_multi(table, origins, tile_image, ph, pw, out):
 def maxpool2(x, C_, out):
     B, H, W, ld = x.shape
     call('pf_maxpool2', x, B, H, W, pad_to(C_, 8), ld, out, out.shape[-1], stream_ptr())
+
+
+def seed_bins(S, nbins, flags, min_depth, max_depth, out):
+    """pf_seed_bins: the seed regressor's fp32 `_net` output S [..., S_ld] (one row per pixel) -> bin centres
+    out [..., nbins].  flags: lib.SEED_NORMED (SeedBinRegressor) | lib.SEED_TO_UNIT ((c - min) / (max - min))."""
+    call('pf_seed_bins', S, S.shape[-1], S.numel() // S.shape[-1], nbins, flags, C.c_float(min_depth),
+         C.c_float(max_depth), out, stream_ptr())
+
+
+def attractor_normed(A, nA, b_prev, flags, min_depth, max_depth, b_out, centers=None):
+    """pf_attractor_normed: A fp32 [B, H, W, A_ld] (the even `_net` channels, ReLU'd), b_prev [B, h, w, nbins] ->
+    b_out [B, H, W, nbins] and, when given, the sorted and clipped metric centres [B, H, W, nbins]."""
+    B, H, W, A_ld = A.shape
+    _, PH, PW, nb = b_prev.shape
+    call('pf_attractor_normed', A, A_ld, nA, b_prev, PH, PW, B, H, W, nb, flags, C.c_float(min_depth),
+         C.c_float(max_depth), b_out, centers, stream_ptr())

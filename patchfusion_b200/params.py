@@ -51,8 +51,6 @@ def branch_hparams(branch_cfg):
     hp['bin_centers_type'] = _get(branch_cfg, 'bin_centers_type', 'softplus')
     if hp['bin_centers_type'] not in ('normed', 'softplus', 'hybrid1', 'hybrid2'):
         raise ValueError("bin_centers_type should be one of 'normed', 'softplus', 'hybrid1', 'hybrid2'")
-    if hp['bin_centers_type'] != 'softplus':
-        raise NotImplementedError("only bin_centers_type='softplus' (every shipped PatchFusion config) is built")
     # config fields that change the reference's arithmetic (zoedepth_v1.py:41-42 constructor defaults): honour the
     # ones the kernels implement, refuse the rest instead of silently computing something else
     hp['attractor_kind'] = _get(branch_cfg, 'attractor_kind', 'sum')
@@ -65,6 +63,16 @@ def branch_hparams(branch_cfg):
         raise NotImplementedError('do_resize=True (depth_anything.py:177-190 resizer) is not built: PatchFusion feeds '
                                   'tiles already at patch_process_shape')
     return hp
+
+
+def normed_seed(bin_centers_type):
+    """the head's seed regressor is SeedBinRegressor (`zoedepth_v1.py:90-105`): ReLU widths normalised and cumulated into centres"""
+    return bin_centers_type in ('normed', 'hybrid1')
+
+
+def normed_attractors(bin_centers_type):
+    """the head's attractors are AttractorLayer (`zoedepth_v1.py:90-105`): normalised centres, sorted and clipped metric output"""
+    return bin_centers_type in ('normed', 'hybrid2')
 
 
 def _f(shape):
@@ -106,9 +114,11 @@ def _metric_head(L, pre, C, hp):
     for i in range(4):
         _conv(L, pre + 'projectors.%d._net.0' % i, 128, C, 1)
         _conv(L, pre + 'projectors.%d._net.2' % i, E, 128, 1)
+    # AttractorLayer emits 2 channels per attractor (`attractor.py:80-85`), AttractorLayerUnnormed one (:157-162)
+    per_attractor = 2 if normed_attractors(hp['bin_centers_type']) else 1
     for i in range(4):
         _conv(L, pre + 'attractors.%d._net.0' % i, 128, E, 1)
-        _conv(L, pre + 'attractors.%d._net.2' % i, hp['n_attractors'][i], 128, 1)
+        _conv(L, pre + 'attractors.%d._net.2' % i, per_attractor * hp['n_attractors'][i], 128, 1)
     L[pre + 'conditional_log_binomial.log_binomial_transform.k_idx'] = ((1, hp['n_bins'], 1, 1), torch.int64, 'buffer')
     L[pre + 'conditional_log_binomial.log_binomial_transform.K_minus_1'] = ((1, 1, 1, 1), torch.float32, 'buffer')
     cin = N_MIDAS_OUT + 1 + E

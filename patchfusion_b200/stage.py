@@ -24,7 +24,8 @@ class PfHead(C.Structure):
     _fields_ = [('seed0', PfLayer), ('seed2', PfLayer), ('seedproj0', PfLayer), ('seedproj2', PfLayer),
                 ('proj0', PfLayer * 4), ('proj2', PfLayer * 4), ('att0', PfLayer * 4), ('att2', PfLayer * 4),
                 ('clb0', PfLayer), ('n_attractors', i32 * 4), ('n_bins', i32), ('bin_embedding_dim', i32),
-                ('attractor_flags', i32), ('has_rel', i32), ('min_temp', f32), ('max_temp', f32)]
+                ('attractor_flags', i32), ('has_rel', i32), ('min_temp', f32), ('max_temp', f32),
+                ('bin_centers_type', i32), ('min_depth', f32), ('max_depth', f32)]
 
 
 class PfBranch(C.Structure):
