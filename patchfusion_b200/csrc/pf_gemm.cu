@@ -1,6 +1,7 @@
 // Implicit-GEMM engine of the PatchFusion hot path (wgmma / TMA / mbarrier, sm_90a).
 //
-// One persistent, warp-specialised kernel serves every dense contraction of the path:
+// One persistent, warp-specialised kernel serves every dense contraction of the path (the plain linear layers run on a
+// ping-pong variant of it, pf_gemm_pp_kernel, further down):
 //   * ViT / Swin linear layers            (`dinov2/layers/attention.py:51,60`, `mlp.py:36-39`, `swin_layers.py:140,162`)
 //   * 1x1 convs (NHWC == plain GEMM)      (`depth_anything/dpt.py:30-38`, metric-head MLPs `localbins_layers.py:84-117`)
 //   * 3x3 stride-1 pad-1 convs over a channel-concat of up to three NHWC sources
@@ -629,11 +630,11 @@ __device__ __forceinline__ void release_stage(uint64_t* bar, int lane) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Phase timeline of pf_gemm_kernel and pf_conv3_halo_kernel (built only with -DPF_GEMM_TIMELINE; pf_gemm_timeline reads
-// it).  One lane per role records clock64 intervals in registers and adds them to g_gemm_timeline when its CTA retires:
+// Phase timeline of pf_gemm_kernel, pf_gemm_pp_kernel and pf_conv3_halo_kernel (built only with -DPF_GEMM_TIMELINE;
+// pf_gemm_timeline reads it).  One lane per role records clock64 intervals in registers and adds them to g_gemm_timeline when its CTA retires:
 // the TMA producer (slots 0-2: tiles, cycles waiting for an empty stage - halo slot or weight stage in the halo kernel -,
 // cycles in its loop) and lane 0 of each consumer warpgroup's first warp (slots 3-7: tiles, cycles waiting for a full
-// stage / halo slot, mainloop cycles including those waits, epilogue cycles, cycles in its loop).  Both kernels add to
+// stage / halo slot, mainloop cycles including those waits, epilogue cycles, cycles in its loop).  All kernels add to
 // the same slots: a reader takes the sums around launches of one kernel and shape.  Every other build compiles the
 // stamps to nothing.
 #ifdef PF_GEMM_TIMELINE
@@ -778,6 +779,218 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_kernel(const __grid_c
     if (lane == 0) bulk_wait0();    // the staging tiles are read (and the writes performed) before the CTA retires
     tl.add(4, tl_start);
     if (lane == 0 && (warp & 3) == 0) tl.flush(3, 5);
+  }
+  __syncthreads();
+  if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Ping-pong GEMM for the plain linear layers (pf_gemm_pp_kernel, d.pp): a_mode 0, one source, N a multiple of 128, and
+// an epilogue of bias -> none / GELU / ReLU with a bf16 bulk store, an fp32 bulk store, the gamma residual reduce-add,
+// or the V^T third of a fused qkv projection.
+//
+// In pf_gemm_kernel both warpgroups finish a tile's mainloop together and then run its epilogue together, so the tensor
+// cores idle for the whole epilogue (about half of a tile's time on the ViT qkv and fc1 linears).  Here consumer
+// warpgroup h owns WHOLE 128 x 128 tiles: tiles 0, 2, 4, ... of the CTA's sequence go to warpgroup 0 and 1, 3, 5, ... to
+// warpgroup 1, and the producer loads their K blocks in that order.  Per k16 step a warpgroup issues two
+// wgmma.m64n128k16 (A rows 0-63 and 64-127, both operands from shared memory), so each B tile is read by one warpgroup
+// only.  Two named barriers hand the tensor cores from one warpgroup to the other: a warpgroup starts a tile's MMAs once
+// the other has issued all of the previous tile's, and while one runs its epilogue the other runs its mainloop.
+// A block_n = 256 work item (the width pf_gemm chooses for the launch) is two consecutive 128-column tiles.
+// A warp's accumulator rows 16w .. 16w + 15 of each 64-row half go through the same fragment-layout epilogue as
+// pf_gemm_kernel's, as "warp" w and w + 4 of a 128-row tile; the V^T tiles store straight from the fragment.
+constexpr int kPpStageBytes = kATileBytes + kPpBN * kBlockK * 2;      // 32 KiB: A 128 x 64 + B 128 x 64
+constexpr int kPpStages = (kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kStageWarp) / kPpStageBytes;
+static_assert(kPpStages == 6, "pf_gemm_pp_kernel operand ring");
+constexpr int kPpTurnBar = 1;        // named barriers 1 and 2: warpgroup 0's and warpgroup 1's turn to issue MMAs
+
+// the two consumer warpgroups (256 threads) meet on named barrier ID: one waits, the other arrives
+template <int ID>
+__device__ __forceinline__ void named_bar_sync256() { asm volatile("bar.sync %0, 256;" ::"n"(ID) : "memory"); }
+template <int ID>
+__device__ __forceinline__ void named_bar_arrive256() { asm volatile("bar.arrive %0, 256;" ::"n"(ID) : "memory"); }
+
+// V^T third of a fused qkv projection, stored from the accumulator fragment: vt[(b * heads + h) * 64 + dd][token].
+// For one column the eight lanes 4i + q (i = 0..7) hold eight consecutive tokens, 16 contiguous bytes of a V^T row
+// (split where the tokens cross an image boundary, m / vt_seq).  Same bias -> activation as the row path, so the same
+// bits.  32-bit offsets keep the accumulators' neighbours in registers.
+template <int S>
+__device__ __forceinline__ void epilogue_tile_vt(const GemmDesc& d, const float (&acc)[S], const TileCoord& c, int warp,
+                                                 int lane) {
+  const int q = lane & 3;
+  int ro[2];               // element offset of this thread's two tokens in V^T row 0 (-1: row past M); the host
+                           // takes this path only when every V^T index fits in 31 bits
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = c.m0 + 16 * warp + (lane >> 2) + 8 * h;
+    const int b = m / d.vt_seq, tok = m - b * d.vt_seq;
+    ro[h] = m < d.M ? b * d.vt_dim * d.vt_seq_pad + tok : -1;
+  }
+  for (int ch = 0; 32 * ch < 2 * S; ++ch) {
+    const int lcol = c.n0 + ch * 32;
+    if (lcol >= d.n_logical) break;
+    float v[16];
+    acc_chunk(ch, acc, v);
+    epi_frag(d, v, lcol + 2 * q, false);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = lcol + 8 * j + 2 * q + e;
+        if (n >= d.n_logical) continue;
+        __nv_bfloat16* vp = d.vt + (n - d.vt_col0) * d.vt_seq_pad;
+        if (ro[0] >= 0) vp[ro[0]] = __float2bfloat16(v[4 * j + e]);
+        if (ro[1] >= 0) vp[ro[1]] = __float2bfloat16(v[4 * j + 2 + e]);
+      }
+    }
+  }
+}
+
+// 64 rows x 128 columns of a pf_gemm_pp_kernel tile: rows 16 warp .. 16 warp + 15 of this consumer warp
+template <int S>
+__device__ __forceinline__ void epilogue_tile_pp(const GemmDesc& d, EpiTma& et, const float (&acc)[S], const TileCoord& c,
+                                                 int warp, int lane) {
+  if (d.vt != nullptr && c.n0 >= d.vt_col0) epilogue_tile_vt(d, acc, c, warp, lane);
+  else if (d.tma_out == 2) epilogue_tile_tma_f32(d, et, acc, c, warp, lane);
+  else epilogue_tile_tma_bf16<64>(d, et, acc, c, warp, lane);
+}
+
+template <bool MC>
+__global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __grid_constant__ GemmKernelParams P) {
+  constexpr int CL = MC ? 2 : 1;
+  extern __shared__ uint8_t smem_raw[];
+  const GemmDesc& d = P.d;
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* stg = smem + kPpStages * kPpStageBytes;   // [kEpiWarps][2][2 KB] staging tiles, 1024-B aligned
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + kEpiWarps * kStageWarp);
+  uint64_t* empty_bar = full_bar + kPpStages;
+
+  // warp-uniform by construction, so the warpgroup / tile / ring state derived from it lives in uniform registers
+  // and the 128 accumulators leave room for the epilogue
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = threadIdx.x & 31;
+  pdl_launch_dependents();
+
+  constexpr int kTmaWarp = kEpiWarps;
+  if (warp == kTmaWarp && lane == 0) {
+    prefetch_tmap(&P.tmA[0]);
+    prefetch_tmap(MC ? &P.tmBh : &P.tmB);
+    // a stage is read by ONE warpgroup: refilled after its 4 warps in every CTA it was multicast to released it
+    for (int s = 0; s < kPpStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4 * CL); }
+    prefetch_tmap(&P.tmOut);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  if (MC) cluster_sync_all();       // the peer's barriers exist before anything is multicast into its shared memory
+  const TileIter it = make_iter(d, P.total_tiles, CL);
+  // this CTA's tile sequence: its work items in schedule order, each split into block_n / 128 tiles (both CTAs of a
+  // cluster walk the same sequence, so their warpgroups stay aligned on the multicast stages)
+  const int sub_log2 = d.block_n == 2 * kPpBN ? 1 : 0;
+  const int items = it.first < it.count ? (it.count - 1 - it.first) / it.step + 1 : 0;
+  const int tiles = items << sub_log2;
+  pdl_wait();                       // predecessor's results are visible from here on
+
+  if (warp >= kEpiWarps) {
+    if (warp == kTmaWarp) {
+      // ===================== TMA producer: the K blocks of tile 0, tile 1, ... =====================
+      GemmTimeline tl;
+      const long long tl_start = tl.now();
+      int stage = 0; uint32_t phase = 0;
+      for (int p = 0; p < tiles; ++p) {
+        TileCoord c = decode_tile(d, it.tile(it.first + (p >> sub_log2) * it.step));
+        c.n0 += (p & sub_log2) * kPpBN;
+        tl.tile();
+        for (int kb = 0; kb < P.k_steps; ++kb) {
+          const long long tl_w = tl.now();
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          tl.add(1, tl_w);
+          uint8_t* sa = smem + stage * kPpStageBytes;
+          uint8_t* sb = sa + kATileBytes;
+          if (elect_one()) {
+            mbar_expect_tx(&full_bar[stage], kPpStageBytes);
+            tma_load_2d(sa, &P.tmA[0], &full_bar[stage], kb * kBlockK, c.m0);
+            if (MC) {
+              constexpr int half_rows = kPpBN / 2;
+              tma_load_2d_mc(sb + it.rank * half_rows * 128, &P.tmBh, &full_bar[stage], kb * kBlockK,
+                             c.n0 + it.rank * half_rows, static_cast<uint16_t>(3));
+            } else {
+              tma_load_2d(sb, &P.tmB, &full_bar[stage], kb * kBlockK, c.n0);
+            }
+          }
+          if (++stage == kPpStages) { stage = 0; phase ^= 1; }
+        }
+      }
+      tl.add(2, tl_start);
+      if (lane == 0) tl.flush(0, 3);
+    }
+  } else {
+    // ===================== consumer warpgroups: every other tile each, mainloops in turn =====================
+    const int wg = warp >> 2, w = warp & 3;
+    EpiTma et;
+    et.tm = &P.tmOut; et.stg_ptr = stg + warp * kStageWarp; et.stg = smem_u32(et.stg_ptr); et.cur = 0;
+    int stage = 0; uint32_t phase = 0;
+    // ring position of the next block this warpgroup reads: skip n blocks (the other warpgroup's tile)
+    auto skip = [&](int n) {
+      stage += n;
+      while (stage >= kPpStages) { stage -= kPpStages; phase ^= 1; }
+    };
+    skip(wg * P.k_steps);
+    GemmTimeline tl;
+    const long long tl_start = tl.now();
+    for (int p = wg; p < tiles; p += 2) {
+      TileCoord c = decode_tile(d, it.tile(it.first + (p >> sub_log2) * it.step));
+      c.n0 += (p & sub_log2) * kPpBN;
+      tl.tile();
+      if (p > 0) {                                          // the other warpgroup has issued tile p - 1's MMAs
+        if (wg == 0) named_bar_sync256<kPpTurnBar>();
+        else named_bar_sync256<kPpTurnBar + 1>();
+      }
+      const long long tl_main = tl.now();
+      // tile rows 0-63 and 64-127, declared per tile: the previous tile's values are dead once its epilogue has read
+      // them (the first wgmma ignores them, scale-d = 0)
+      float acc0[kPpBN / 2], acc1[kPpBN / 2];
+#pragma unroll
+      for (int i = 0; i < kPpBN / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+      uint32_t accum = 0;
+      int prev = 0;                                         // stage of the previous K block
+      for (int kb = 0; kb < P.k_steps; ++kb) {
+        const long long tl_w = tl.now();
+        mbar_wait(&full_bar[stage], phase);
+        tl.add(1, tl_w);
+        const uint32_t sa = smem_u32(smem + stage * kPpStageBytes);
+        const uint64_t adesc = wgmma_desc_k128(sa);
+        const uint64_t adesc1 = wgmma_desc_k128(sa + 64 * 128);
+        const uint64_t bdesc = wgmma_desc_k128(sa + kATileBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          Wgmma<kPpBN>::ss(acc0, adesc + 2 * k, bdesc + 2 * k, accum | k);
+          Wgmma<kPpBN>::ss(acc1, adesc1 + 2 * k, bdesc + 2 * k, accum | k);
+        }
+        wgmma_commit();
+        accum = 1;
+        wgmma_wait<1>();                                    // the group of block kb - 1 is done ...
+        if (kb > 0) release_stage<CL>(&empty_bar[prev], lane);   // ... and it was the last reader of its stage
+        prev = stage;
+        skip(1);
+      }
+      if (p + 1 < tiles) {                                  // the other warpgroup's turn
+        if (wg == 0) named_bar_arrive256<kPpTurnBar + 1>();
+        else named_bar_arrive256<kPpTurnBar>();
+      }
+      wgmma_wait<0>();                                      // the tile's last block is done: its stage is free
+      release_stage<CL>(&empty_bar[prev], lane);
+      skip(P.k_steps);                                      // tile p + 1 is the other warpgroup's
+      tl.add(2, tl_main);
+      const long long tl_epi = tl.now();
+      epilogue_tile_pp(d, et, acc0, c, w, lane);
+      epilogue_tile_pp(d, et, acc1, c, w + 4, lane);
+      __syncwarp();
+      tl.add(3, tl_epi);
+    }
+    if (lane == 0) bulk_wait0();    // the staging tiles are read (and the writes performed) before the CTA retires
+    tl.add(4, tl_start);
+    if (lane == 0 && w == 0) tl.flush(3, 5);
   }
   __syncthreads();
   if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
@@ -1106,6 +1319,7 @@ static KernelFn gemm_kernel_mc(int bn) {
   }
 }
 static KernelFn gemm_kernel(bool mc, int bn) { return mc ? gemm_kernel_mc<true>(bn) : gemm_kernel_mc<false>(bn); }
+static KernelFn gemm_pp_kernel(bool mc) { return mc ? pf_gemm_pp_kernel<true> : pf_gemm_pp_kernel<false>; }
 
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
                 const CUtensorMap* tmOut, cudaStream_t stream) {
@@ -1116,6 +1330,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     for (bool mc : {false, true})
       for (int bn : kGemmWidths)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_kernel(mc, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    for (bool mc : {false, true})
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_pp_kernel(mc), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (int cl : {1, 2, 4})
       for (int bn : {32, 64, 128, 192})
         if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
@@ -1186,9 +1402,12 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     }
     if (le != cudaSuccess) return set_error("pf_conv3_halo_kernel launch: %s", cudaGetErrorString(le));
   } else {
-    const KernelFn gk = gemm_kernel(tmBh != nullptr, d.block_n);
+    if (d.pp && (d.block_n % kPpBN != 0 || d.num_src != 1 || d.a_mode != 0 || !d.tma_out))
+      return set_error("gemm: the ping-pong kernel takes plain linear layers at block_n 128 / 256 (block_n %d)", d.block_n);
+    const KernelFn gk = d.pp ? gemm_pp_kernel(tmBh != nullptr) : gemm_kernel(tmBh != nullptr, d.block_n);
     if (gk == nullptr) return set_error("gemm: block_n %d (32, 64, 96, 128, 192 or 256)", d.block_n);
-    const size_t smem = 1024 + static_cast<size_t>(gemm_stages(d.block_n)) * gemm_stage_bytes(d.block_n) +
+    const size_t smem = 1024 + (d.pp ? static_cast<size_t>(kPpStages) * kPpStageBytes
+                                     : static_cast<size_t>(gemm_stages(d.block_n)) * gemm_stage_bytes(d.block_n)) +
                         kEpiWarps * kStageWarp + kBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
@@ -1208,11 +1427,11 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     } else {
       le = launch_pdl(gk, dim3(grid), dim3(kGemmThreads), smem, stream, P);
     }
-    if (le != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(le));
+    if (le != cudaSuccess) return set_error("%s launch: %s", d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel", cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(e));
-  count_launch(d.halo ? "pf_conv3_halo_kernel" : "pf_gemm_kernel");
+  count_launch(d.halo ? "pf_conv3_halo_kernel" : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"));
   return 0;
 }
 

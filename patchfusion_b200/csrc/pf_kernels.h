@@ -45,6 +45,7 @@ struct GemmDesc {
   float rs_sy[3], rs_sx[3];
   int rs_any;
   int tma_out;           // pf_gemm_kernel epilogue through shared memory + TMA: 0 direct, 1 bf16 output, 2 fp32 output / residual stream
+  int pp;                // plain linear layer through pf_gemm_pp_kernel (128 x 128 tiles, one per consumer warpgroup)
 };
 
 int set_error(const char* fmt, ...);
@@ -89,7 +90,12 @@ int check_launch(const char* what);
 // registers)
 constexpr int kGemmWidths[] = {32, 64, 96, 128, 192, 256};
 
+// n-tile width of pf_gemm_pp_kernel (d.pp): each consumer warpgroup owns whole 128 x 128 tiles; a block_n = 256 work
+// item is two of them
+constexpr int kPpBN = 128;
+
 // tmBh != nullptr selects the weight-multicast variant (clusters of 2 CTAs): a {64, block_n / 2} box map of the weights
+// ({64, 128} and {64, 64} boxes for d.pp)
 // tmOut: output tensor map when d.tma_out != 0
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
                 const CUtensorMap* tmOut, cudaStream_t stream);
