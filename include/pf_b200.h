@@ -110,6 +110,14 @@ typedef struct pf_gemm_desc {
    * conv reads THROUGH the resample to (H, W); the up-sampled tensor is never written to memory - a producer warp of
    * the halo-tile kernel interpolates each 18 x 10 pixel halo straight into the swizzled operand tile. */
   int32_t rs_h[3], rs_w[3];
+  /* E4M3 operands (a_e4m3 != 0; 3x3 halo-tile convs with materialised sources and a plain bf16 output only): a_ptr[0]
+   * is ONE e4m3 NHWC map [NB, H, W, a_ld[0] bytes] holding the num_src sources back to back, each padded to 64 channels
+   * (pf_quantize_e4m3_tiles); a_c[] still give the sources' channels.  w_ptr is an e4m3 panel (pf_pack_weight_e4m3).
+   * The epilogue computes act(fl(acc * fl(s_a[img] * s_w[n])) + bias[n]): s_a one fp32 scale per image of the batch,
+   * s_w one per output channel. */
+  int32_t a_e4m3;
+  const float* s_a;
+  const float* s_w;
 } pf_gemm_desc;
 
 int pf_gemm(pf_gemm_desc* desc, void* stream);
@@ -123,6 +131,31 @@ int pf_pack_weight(const float* w, int32_t N, int32_t N_pad, int32_t num_src, co
 /* ConvTranspose2d(k==s) weight [Cin, Cout, k, k] -> [k*k*Cp, Cin_pad64] bf16, Cp = pad32(Cout),
  * row = (ky*k + kx)*Cp + co (rows co >= Cout are zero).  Use with pf_gemm ps=k, ps_cout=Cout, N=k*k*Cp. */
 int pf_pack_weight_convT(const float* w, int32_t Cin, int32_t Cout, int32_t k, void* dst, void* stream);
+
+/* ---- E4M3 (FP8) operands of the Guided-Fusion U-Net's 3x3 convs (model config fusion_precision = 'fp8') ----------
+ * Rounding rule shared by both entry points, all in IEEE fp32 without contraction:
+ *   amax  = max |v| over the group (a NaN anywhere makes it NaN, an infinity makes it +inf)
+ *   r     = 448 / amax, or 0 when amax == 0
+ *   q     = e4m3_rn(v * r)    round to nearest even to float8_e4m3fn (torch.float8_e4m3fn; |v * r| <= 448, so no
+ *                             saturation happens; the sign of zero is kept; NaN stays NaN)
+ *   scale = amax / 448        so that v ~= q * scale; an all-zero group gets scale 0 and q = 0
+ * Non-finite data propagate: a group holding NaN gets scale NaN and q NaN everywhere (r = NaN); a group holding an
+ * infinity gets scale +inf, q = 0 for its finite values and NaN for the infinities (r = 0).  The conv's accumulator times
+ * such a scale is NaN; what the activation makes of a NaN is as in the bf16 path (ReLU's fmaxf returns 0). */
+/* pf_pack_weight's panel and K order (source, tap, 64-channel chunk; pad channels and rows >= N zero) with one group
+ * per output channel: v = w[n, ...] * scale[n] (BatchNorm folded first, when scale != NULL), dst e4m3 [N_pad, Ktot],
+ * s_w[n] (n < N) the channel's scale. */
+int pf_pack_weight_e4m3(const float* w, int32_t N, int32_t N_pad, int32_t num_src, const int32_t* src_c, int32_t taps,
+                        const float* scale, void* dst, float* s_w, void* stream);
+/* One group per TILE (batch index t of the U-Net maps) over all of a conv's sources: src[i] (host array of device
+ * pointers) is a bf16 NHWC map [T, H, W, src_ld[i]] of which the first src_c[i] channels are read (src_ld[i] a multiple
+ * of 8 >= src_c[i], 16-byte aligned).  out: e4m3 [T, H, W, Kc], Kc = sum_i 64 ceil(src_c[i] / 64), the sources back to
+ * back with zero pad channels (the map pf_gemm reads with a_e4m3); s_a[t] the tile's scale.  Two launches: per-block
+ * partial maxima into `partial` (T * PF_QUANT_PARTS floats), then the scales and the map.  A max does not depend on
+ * the order it is taken in, so the result is deterministic and tile t's bytes depend on tile t's data only. */
+#define PF_QUANT_PARTS 32
+int pf_quantize_e4m3_tiles(int32_t num_src, const void* const* src, const int32_t* src_c, const int32_t* src_ld,
+                           int32_t T, int32_t H, int32_t W, float* partial, void* out, float* s_a, void* stream);
 
 /* ---- ViT pieces --------------------------------------------------------------------------------------------- */
 /* LayerNorm over the last dim, fp32 in -> bf16 out (dinov2/layers/block.py:84,87; vision_transformer.py:311;
@@ -342,6 +375,12 @@ typedef struct pf_layer {
   const float* w2;          /* optional trailing 1x1 layer fused into the epilogue: fp32 [n2, N] */
   const float* b2;          /* [n2] or NULL */
   int32_t n2;
+  /* FP8 (3x3 convs of the Guided-Fusion U-Net, fusion_precision = 'fp8'): when w_scale != NULL the conv quantizes its
+   * input per tile (pf_quantize_e4m3_tiles) and runs on the e4m3 panel w8 with per-channel scales w_scale
+   * (pf_pack_weight_e4m3).  w (bf16) may then be NULL unless the conv can run through the fused resample
+   * (PF_OPT_FUSED_RESAMPLE), which has no materialised input to quantize and stays bf16. */
+  const void* w8;
+  const float* w_scale;
 } pf_layer;
 
 typedef struct pf_vit_block {             /* dinov2/layers/block.py:82-107 */

@@ -140,8 +140,8 @@ static int encode(CUtensorMap* out, const void* ptr, int rank, const uint64_t* d
     if (gstr[i] & 15) return set_error("tensor map: stride %d (%llu B) not a multiple of 16", i, (unsigned long long)gstr[i]);
   }
   // rows of 128 bytes: SWIZZLE_128B (every operand tile and most staging tiles); rows of 64 bytes (the 32-column bf16
-  // staging tiles of the halo conv epilogue): SWIZZLE_64B.  The box is part of the cache key, so the mode is too.
-  const uint32_t row_bytes = box[0] * (dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2);
+  // staging tiles of the halo conv epilogue, the e4m3 operand tiles of its FP8 instantiation): SWIZZLE_64B.  The box is part of the cache key, so the mode is too.
+  const uint32_t row_bytes = box[0] * (dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : (dt == CU_TENSOR_MAP_DATA_TYPE_UINT8 ? 1 : 2));
   const CUtensorMapSwizzle swz = row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B;
   CUresult r = fn(out, dt, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -185,6 +185,21 @@ int tmap_4d_nhwc_bf16(CUtensorMap* out, const void* ptr, uint64_t C, uint64_t W,
   uint64_t str[3] = {ld * 2, ld * 2 * W, ld * 2 * W * H};
   uint32_t box[4] = {box_c, box_w, box_h, 1};
   return encode(out, ptr, 4, dims, str, box);
+}
+
+int tmap_2d_u8(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld, uint32_t box_cols,
+               uint32_t box_rows) {
+  uint64_t dims[2] = {cols, rows};
+  uint64_t str[1] = {ld};
+  uint32_t box[2] = {box_cols, box_rows};
+  return encode(out, ptr, 2, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+}
+int tmap_4d_nhwc_u8(CUtensorMap* out, const void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N, uint64_t ld,
+                    uint32_t box_c, uint32_t box_w, uint32_t box_h) {
+  uint64_t dims[4] = {C, W, H, N};
+  uint64_t str[3] = {ld, ld * W, ld * W * H};
+  uint32_t box[4] = {box_c, box_w, box_h, 1};
+  return encode(out, ptr, 4, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_UINT8);
 }
 
 // ---------------------------------------------------------------------------------------------- weight packing
@@ -231,6 +246,157 @@ __global__ void pack_convT_kernel(const float* __restrict__ w, int Cin, int Cout
   float v = 0.0f;
   if (ci < Cin && co < Cout) v = w[(static_cast<long long>(ci) * Cout + co) * k * k + tap];   // [Cin][Cout][ky][kx]
   dst[idx] = __float2bfloat16(v);
+}
+
+// ---------------------------------------------------------------------------------------------- E4M3 quantization
+// The arithmetic pf_pack_weight_e4m3 / pf_quantize_e4m3_tiles document in pf_b200.h, in IEEE fp32 with no contraction.
+// e4m3_rn: cvt.rn.satfinite (round to nearest even; |v| <= 448 by construction, NaN -> NaN)
+__device__ __forceinline__ uint32_t e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// max of |x| that propagates NaN (fmaxf would drop it)
+__device__ __forceinline__ float nanmax(float a, float b) { return a != a ? a : (b != b ? b : fmaxf(a, b)); }
+__device__ __forceinline__ float e4m3_ratio(float amax) { return amax == 0.f ? 0.f : __fdiv_rn(448.f, amax); }
+
+__device__ __forceinline__ float block_nanmax(float m) {
+  __shared__ float red[32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = nanmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+  if (threadIdx.x < 32) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = nanmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (threadIdx.x == 0) red[0] = m;
+  }
+  __syncthreads();
+  m = red[0];
+  __syncthreads();
+  return m;
+}
+
+// one block per panel row: amax of the BN-folded fp32 row, then the row's Ktot bytes in pack_weight_kernel's K order
+__global__ void pack_weight_e4m3_kernel(const float* __restrict__ w, int N, int num_src, int c0, int c1, int c2, int taps,
+                                        const float* __restrict__ scale, uint8_t* __restrict__ dst, float* __restrict__ s_w,
+                                        int Ktot) {
+  const int n = blockIdx.x;
+  const int cs[3] = {c0, c1, c2};
+  const int ctot = c0 + (num_src > 1 ? c1 : 0) + (num_src > 2 ? c2 : 0);
+  const long long row = static_cast<long long>(ctot) * taps;
+  float m = 0.f;
+  if (n < N) {
+    const float sc = scale ? scale[n] : 1.f;
+    for (long long i = threadIdx.x; i < row; i += blockDim.x) {
+      const float v = scale ? __fmul_rn(w[n * row + i], sc) : w[n * row + i];
+      m = nanmax(m, fabsf(v));
+    }
+  }
+  const float amax = block_nanmax(m);
+  const float r = e4m3_ratio(amax);
+  if (n < N && threadIdx.x == 0) s_w[n] = __fdiv_rn(amax, 448.f);
+  for (int k = 2 * threadIdx.x; k < Ktot; k += 2 * blockDim.x) {
+    float v[2] = {0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      int cbase = 0, kbase = 0;
+      for (int s = 0; s < num_src; ++s) {
+        const int cp = (cs[s] + 63) / 64 * 64, seg = taps * cp;
+        if (k + e < kbase + seg) {
+          const int kk = k + e - kbase, tap = kk / cp, c = kk - tap * cp;
+          if (n < N && c < cs[s]) {
+            float x = w[(static_cast<long long>(n) * ctot + cbase + c) * taps + tap];
+            if (scale) x = __fmul_rn(x, scale[n]);
+            v[e] = __fmul_rn(x, r);
+          }
+          break;
+        }
+        kbase += seg;
+        cbase += cs[s];
+      }
+    }
+    *reinterpret_cast<uint16_t*>(dst + static_cast<long long>(n) * Ktot + k) = static_cast<uint16_t>(e4m3x2(v[0], v[1]));
+  }
+}
+
+// Activation sources of one conv: their bf16 maps, logical channels, row pitches, and where each 64-padded segment
+// starts in the e4m3 map
+struct QuantSrc {
+  const __nv_bfloat16* p[3];
+  int c[3], ld[3], koff[3];
+  int ns, kc;        // sources, channels of the e4m3 map
+};
+constexpr int kQuantParts = PF_QUANT_PARTS;
+static_assert(kQuantParts == 32, "quant_write_kernel reduces the partial maxima with one warp");
+
+// launch 1: partial[t][b] = NaN-propagating max |x| over block b's share of tile t's pixels and logical channels
+__global__ void quant_amax_kernel(QuantSrc q, long long hw, float* __restrict__ partial) {
+  const int t = blockIdx.y;
+  int gs[3], g = 0;                                        // 8-channel groups per pixel, per source and in all
+  for (int s = 0; s < q.ns; ++s) { gs[s] = (q.c[s] + 7) / 8; g += gs[s]; }
+  const long long items = hw * g;
+  float m = 0.f;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < items;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long px = i / g;
+    int j = static_cast<int>(i - px * g), s = 0;
+    while (j >= gs[s]) { j -= gs[s]; ++s; }
+    const uint4 u = __ldg(reinterpret_cast<const uint4*>(q.p[s] + (t * hw + px) * q.ld[s] + 8 * j));
+    const uint32_t wv[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      if (8 * j + e < q.c[s]) {
+        const float x = __uint_as_float(e & 1 ? (wv[e >> 1] & 0xffff0000u) : (wv[e >> 1] << 16));
+        m = nanmax(m, fabsf(x));
+      }
+    }
+  }
+  m = block_nanmax(m);
+  if (threadIdx.x == 0) partial[t * kQuantParts + blockIdx.x] = m;
+}
+
+// launch 2: amax_t from the partials (every block of the tile reduces the same values: identical result), s_a[t], and
+// the e4m3 map [T, H, W, kc]: 8 output channels per thread, zeros in the pad channels of each segment
+__global__ void quant_write_kernel(QuantSrc q, long long hw, const float* __restrict__ partial, uint8_t* __restrict__ out,
+                                   float* __restrict__ s_a) {
+  const int t = blockIdx.y;
+  __shared__ float s_amax;
+  if (threadIdx.x < 32) {
+    float m = nanmax(partial[t * kQuantParts + threadIdx.x], 0.f);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = nanmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (threadIdx.x == 0) s_amax = m;
+  }
+  __syncthreads();
+  const float amax = s_amax;
+  const float r = e4m3_ratio(amax);
+  if (blockIdx.x == 0 && threadIdx.x == 0) s_a[t] = __fdiv_rn(amax, 448.f);
+  const int g = q.kc / 8;
+  const long long items = hw * g;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < items;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long px = i / g;
+    const int k = 8 * static_cast<int>(i - px * g);
+    int s = q.ns - 1;
+    while (s > 0 && k < q.koff[s]) --s;
+    const int c = k - q.koff[s];
+    uint32_t lo = 0, hi = 0;
+    if (c < q.c[s]) {
+      const uint4 u = __ldg(reinterpret_cast<const uint4*>(q.p[s] + (t * hw + px) * q.ld[s] + c));
+      const uint32_t wv[4] = {u.x, u.y, u.z, u.w};
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float x = __uint_as_float(e & 1 ? (wv[e >> 1] & 0xffff0000u) : (wv[e >> 1] << 16));
+        v[e] = c + e < q.c[s] ? __fmul_rn(x, r) : 0.f;
+      }
+      lo = e4m3x2(v[0], v[1]) | (e4m3x2(v[2], v[3]) << 16);
+      hi = e4m3x2(v[4], v[5]) | (e4m3x2(v[6], v[7]) << 16);
+    }
+    *reinterpret_cast<uint2*>(out + (t * hw + px) * q.kc + k) = make_uint2(lo, hi);
+  }
 }
 
 }  // namespace pf
@@ -287,6 +453,49 @@ int pf_pack_weight(const float* w, int32_t N, int32_t N_pad, int32_t num_src, co
   return check_launch("pack_weight_kernel");
 }
 
+int pf_pack_weight_e4m3(const float* w, int32_t N, int32_t N_pad, int32_t num_src, const int32_t* src_c, int32_t taps,
+                        const float* scale, void* dst, float* s_w, void* stream) {
+  if (num_src < 1 || num_src > 3 || (taps != 1 && taps != 9) || N < 1 || N_pad < N || !w || !dst || !s_w)
+    return set_error("pf_pack_weight_e4m3: bad arguments");
+  int c[3] = {src_c[0], num_src > 1 ? src_c[1] : 0, num_src > 2 ? src_c[2] : 0};
+  int Ktot = 0;
+  for (int s = 0; s < num_src; ++s) Ktot += taps * ((c[s] + 63) / 64 * 64);
+  pack_weight_e4m3_kernel<<<N_pad, 256, 0, static_cast<cudaStream_t>(stream)>>>(w, N, num_src, c[0], c[1], c[2], taps,
+                                                                                 scale, static_cast<uint8_t*>(dst), s_w, Ktot);
+  return check_launch("pack_weight_e4m3_kernel");
+}
+
+int pf_quantize_e4m3_tiles(int32_t num_src, const void* const* src, const int32_t* src_c, const int32_t* src_ld,
+                           int32_t T, int32_t H, int32_t W, float* partial, void* out, float* s_a, void* stream) {
+  if (num_src < 1 || num_src > 3 || !src || !src_c || !src_ld || T < 1 || H < 1 || W < 1 || !partial || !out || !s_a)
+    return set_error("pf_quantize_e4m3_tiles: bad arguments");
+  QuantSrc q;
+  memset(&q, 0, sizeof(q));
+  q.ns = num_src;
+  for (int s = 0; s < num_src; ++s) {
+    q.p[s] = static_cast<const __nv_bfloat16*>(src[s]);
+    q.c[s] = src_c[s]; q.ld[s] = src_ld[s]; q.koff[s] = q.kc;
+    if (!src[s] || src_c[s] < 1 || src_ld[s] < (src_c[s] + 7) / 8 * 8 || src_ld[s] % 8 || reinterpret_cast<uintptr_t>(src[s]) & 15)
+      return set_error("pf_quantize_e4m3_tiles: source %d: channels %d, ld %d (a multiple of 8 covering them), 16-byte aligned",
+                       s, src_c[s], src_ld[s]);
+    q.kc += (src_c[s] + 63) / 64 * 64;
+  }
+  if (reinterpret_cast<uintptr_t>(out) & 7) return set_error("pf_quantize_e4m3_tiles: output not 8-byte aligned");
+  const long long hw = static_cast<long long>(H) * W;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  note_work(0.0, "amax e4m3 T%d %dx%d K%d", T, H, W, q.kc);
+  quant_amax_kernel<<<dim3(kQuantParts, T), 256, 0, st>>>(q, hw, partial);
+  if (int rc = check_launch("quant_amax_kernel")) return rc;
+  // enough blocks to fill the GPU whatever T is
+  const long long items = hw * (q.kc / 8);
+  long long bx = (items + 255) / 256;
+  const long long cap = (4LL * sm_count() + T - 1) / T;
+  if (bx > cap) bx = cap < 1 ? 1 : cap;
+  note_work(0.0, "quantize e4m3 T%d %dx%d K%d", T, H, W, q.kc);
+  quant_write_kernel<<<dim3(static_cast<unsigned>(bx), T), 256, 0, st>>>(q, hw, partial, static_cast<uint8_t*>(out), s_a);
+  return check_launch("quant_write_kernel");
+}
+
 int pf_pack_weight_convT(const float* w, int32_t Cin, int32_t Cout, int32_t k, void* dst, void* stream) {
   int Kp = (Cin + 63) / 64 * 64;
   long long total = static_cast<long long>(k) * k * ((Cout + 31) / 32 * 32) * Kp;
@@ -314,6 +523,10 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   if (u->taps == 9 && u->a_mode != 1) return set_error("pf_gemm: 3x3 window needs a_mode 1");
   if (u->N <= 0) return set_error("pf_gemm: N %d", u->N);
   if (u->out_ld % 8 || u->out_col0 % 8) return set_error("pf_gemm: out_ld/out_col0 must be multiples of 8");
+  const bool e4m3 = u->a_e4m3 != 0;
+  if (e4m3 && (u->a_mode != 1 || u->taps != 9 || u->bh != 0 || u->bw != 0 || getenv("PF_B200_NO_HALO") != nullptr ||
+               u->rs_h[0] || u->rs_h[1] || u->rs_h[2] || !u->s_a || !u->s_w))
+    return set_error("pf_gemm: e4m3 operands take the 3x3 halo-tile conv with materialised sources and s_a / s_w");
   GemmDesc d;
   memset(&d, 0, sizeof(d));
   d.num_src = u->num_src; d.a_mode = u->a_mode; d.taps = u->taps;
@@ -367,7 +580,16 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
         if (reinterpret_cast<uintptr_t>(u->a_ptr[s]) & 15) return set_error("pf_gemm: resampled source %d not 16-byte aligned", s);
         continue;
       }
-      if (tmap_4d_nhwc_bf16(&tmA[s], u->a_ptr[s], u->a_c[s], u->W, u->H, u->NB, u->a_ld[s], 64, 10, 18)) return 1;
+      if (e4m3) {
+        // one e4m3 map holds every source, each padded to 64 channels (pf_quantize_e4m3_tiles); a_ld[0] in bytes
+        int kc = 0;
+        for (int j = 0; j < u->num_src; ++j) kc += d.chunks[j] * 64;
+        if (u->a_ld[0] < kc || u->a_ld[0] % 16) return set_error("pf_gemm: e4m3 map pitch %d < %d channels", u->a_ld[0], kc);
+        if (s == 0 && tmap_4d_nhwc_u8(&tmA[0], u->a_ptr[0], kc, u->W, u->H, u->NB, u->a_ld[0], 64, 10, 18)) return 1;
+        tmA[s] = tmA[0];
+      } else if (tmap_4d_nhwc_bf16(&tmA[s], u->a_ptr[s], u->a_c[s], u->W, u->H, u->NB, u->a_ld[s], 64, 10, 18)) {
+        return 1;
+      }
       if (first_plain < 0) first_plain = s;
     }
     for (int s = 0; s < u->num_src; ++s)       // placeholder maps for the resampled sources (never dereferenced)
@@ -418,7 +640,12 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   }
   d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
   u->block_n = bn; u->n_tiles = d.n_tiles;
-  if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) return 1;
+  if (e4m3) {
+    if (tmap_2d_u8(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) return 1;
+    d.a_e4m3 = 1; d.s_a = u->s_a; d.s_w = u->s_w;
+  } else if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) {
+    return 1;
+  }
   d.bias = u->bias; d.act = u->act;
   d.res1 = static_cast<const __nv_bfloat16*>(u->res1);
   d.res2 = static_cast<const __nv_bfloat16*>(u->res2);
@@ -464,7 +691,9 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   d.halo_cl = halo ? cl : 1;
   const bool mc = cl > 1;
   CUtensorMap tmBh;
-  if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)) return 1;
+  if (mc && (e4m3 ? tmap_2d_u8(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)
+                  : tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)))
+    return 1;
   // Epilogue through shared memory + TMA: plain bf16 outputs in 64-column groups (32-column groups in the halo kernel at
   // block_n 32), and, in pf_gemm_kernel only, fp32 outputs and the fp32 residual stream (x += gamma * v) in 32-column
   // chunks.  Halo convs reading a fused resample keep the direct stores.  PF_OPT_TMA_EPILOGUE = 0 keeps the direct
@@ -510,6 +739,10 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
     if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, kPpBN)) return 1;
     if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, kPpBN / 2)) return 1;
   }
+  // the FP8 instantiation has only the plain-output fragment epilogue (bias + activation -> stmatrix -> bulk store)
+  if (e4m3 && d.tma_out != 1)
+    return set_error("pf_gemm: an e4m3 conv needs the bulk-store epilogue: a plain bf16 output, 16-byte aligned, and "
+                     "PF_OPT_TMA_EPILOGUE on");
   return gemm_launch(d, tmA, tmB, mc ? &tmBh : nullptr, d.tma_out ? &tmOut : nullptr, static_cast<cudaStream_t>(stream));
 }
 

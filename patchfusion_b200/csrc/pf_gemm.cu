@@ -449,10 +449,23 @@ __device__ __forceinline__ void epi_tma_store(const GemmDesc& d, const EpiTma& e
 // matrices per 16 columns (column octet o, rows 0-7 / 8-15), written by stmatrix: lane l addresses row r = l & 15 of
 // octet pair member l >> 4, 16-byte piece o ^ (r & 7) of the 128-byte row, or o ^ ((r >> 1) & 3) of the 64-byte row
 // (the swizzle XORs address bits 4-6 with bits 7-9, or bits 4-5 with bits 7-8).
-template <int G, int S>
+// SC (the FP8 halo conv): the accumulator is first multiplied by s_a[img] * s_w[column] (__fmul_rn each, so the bias add
+// that follows is a separate rounding: v = fl(fl(acc * fl(s_a * s_w)) + bias)).
+__device__ __forceinline__ void epi_dequant(const GemmDesc& d, float (&v)[16], int col, float sa) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 w = epi_vec2(d.s_w, col + 8 * j, d.n_logical);
+    const float kx = __fmul_rn(sa, w.x), ky = __fmul_rn(sa, w.y);
+    v[4 * j] = __fmul_rn(v[4 * j], kx); v[4 * j + 1] = __fmul_rn(v[4 * j + 1], ky);
+    v[4 * j + 2] = __fmul_rn(v[4 * j + 2], kx); v[4 * j + 3] = __fmul_rn(v[4 * j + 3], ky);
+  }
+}
+template <int G, int S, bool SC = false>
 __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                        const TileCoord& c, int warp, int lane) {
   static_assert(G == 64 || G == 32, "group width");
+  float sa = 0.f;
+  if constexpr (SC) sa = c.img < d.NB ? __ldg(d.s_a + c.img) : 0.f;   // img >= NB: a cluster's phantom tile
   const int oct = lane >> 4;
   const uint32_t lane_off = (lane & 15) * (2 * G);
   const int swz = G == 64 ? (lane & 7) : ((lane >> 1) & 3);
@@ -464,6 +477,7 @@ __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma
     for (int h = 0; h < G / 32; ++h) {
       float v[16];
       acc_chunk(G / 32 * g + h, acc, v);
+      if constexpr (SC) epi_dequant(d, v, lcol + 32 * h + 2 * (lane & 3), sa);
       epi_frag(d, v, lcol + 32 * h + 2 * (lane & 3), false);
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
@@ -1017,20 +1031,35 @@ constexpr int kHaloW = 10, kHaloH = 18;
 constexpr int kHaloBytes = kHaloW * kHaloH * 128;          // 23040
 constexpr int kHaloSlot = 24 * 1024;                        // 1024-B aligned slot
 constexpr int kHaloSlots = 3;
+// The FP8 instantiation (F8: e4m3 operands) keeps the 64-channel chunk, so a pixel of the halo is a 64-byte row
+// (SWIZZLE_64B): 11520-byte halo tiles in 12 KB slots and BN x 64-byte weight tap tiles.  What it saves goes to the
+// weight ring.  EB = bytes per element.
+__host__ __device__ constexpr int halo_slot(bool f8) { return f8 ? 12 * 1024 : kHaloSlot; }
+__host__ __device__ constexpr int halo_bytes(bool f8) { return f8 ? kHaloW * kHaloH * 64 : kHaloBytes; }
 // shared memory left for the weight ring next to the halo slots, the epilogue staging tiles and barriers
-constexpr int kHaloBBytes = kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kStageWarp - kHaloSlots * kHaloSlot;
+__host__ __device__ constexpr int halo_bbytes(bool f8) {
+  return kMaxSmem - 1024 /*align*/ - kBarBytes - kEpiWarps * kStageWarp - kHaloSlots * halo_slot(f8);
+}
+constexpr int kHaloBBytes = halo_bbytes(false);
 // taps per weight stage: amortise the per-stage barrier round trip over several taps while two stages still fit
-__host__ __device__ constexpr int halo_kc(int bn) {
-  return 2 * 9 * bn * kBlockK * 2 <= kHaloBBytes ? 9 : (2 * 3 * bn * kBlockK * 2 <= kHaloBBytes ? 3 : 1);
+__host__ __device__ constexpr int halo_kc(int bn, bool f8 = false) {
+  return 2 * 9 * bn * kBlockK * (f8 ? 1 : 2) <= halo_bbytes(f8) ? 9
+                                                                 : (2 * 3 * bn * kBlockK * (f8 ? 1 : 2) <= halo_bbytes(f8) ? 3 : 1);
 }
 // weight ring depth: as many stages of halo_kc taps as fit (at least two by the choice of halo_kc), at most six
-__host__ __device__ constexpr int halo_stages(int bn) {
-  return kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) < 6 ? kHaloBBytes / (halo_kc(bn) * bn * kBlockK * 2) : 6;
+__host__ __device__ constexpr int halo_stages(int bn, bool f8 = false) {
+  return halo_bbytes(f8) / (halo_kc(bn, f8) * bn * kBlockK * (f8 ? 1 : 2)) < 6
+             ? halo_bbytes(f8) / (halo_kc(bn, f8) * bn * kBlockK * (f8 ? 1 : 2))
+             : 6;
 }
 // The second staging tile per warp costs no weight stage and no taps per stage at any width
 static_assert(halo_kc(32) == 9 && halo_stages(32) == 3 && halo_kc(64) == 3 && halo_stages(64) == 5 &&
                   halo_kc(128) == 3 && halo_stages(128) == 2 && halo_kc(192) == 1 && halo_stages(192) == 5,
               "halo weight ring");
+static_assert(halo_kc(32, true) == 9 && halo_stages(32, true) == 6 && halo_kc(64, true) == 9 && halo_stages(64, true) == 4 &&
+                  halo_kc(128, true) == 9 && halo_stages(128, true) == 2 && halo_kc(192, true) == 3 &&
+                  halo_stages(192, true) == 4,
+              "FP8 halo weight ring");
 
 
 // ---- fused bilinear resample (align_corners=True) of a halo-kernel source -------------------------------------------
@@ -1097,22 +1126,37 @@ __device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&f
 #pragma unroll
   for (int k = 0; k < kBlockK / 16; ++k) ldmatrix_x4(ra + (((2 * k + (lane >> 4)) ^ sw) << 4), fa[k]);
 }
+// FP8: the row is a 64-byte e4m3 halo pixel, k32 step k is 16-byte chunks 2k, 2k + 1 (SWIZZLE_64B: chunk j of the row at
+// address a sits at j ^ ((a >> 7) & 3)).  The .b16 fragment of a 32-byte k slice is the k32 e4m3 A fragment (Wgmma8).
+__device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&fa)[2][4]) {
+  const uint32_t sw = (ra >> 7) & 3;
+#pragma unroll
+  for (int k = 0; k < 2; ++k) ldmatrix_x4(ra + (((2 * k + (lane >> 4)) ^ sw) << 4), fa[k]);
+}
 
 // CL > 1: clusters of CL (2 or 4) CTAs take CL m-tiles (pixel tiles) of the SAME n-tile; each CTA fetches 1/CL of the rows
 // of every weight tile and multicasts it into all of them.  The weights are ~90 % of this kernel's L2 -> SM traffic (one
 // 23 KB halo against nine 4-24 KB tap tiles per 64-channel chunk).
-template <int CL, int BN>
-__global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __grid_constant__ GemmKernelParams P) {
+//
+// F8: the E4M3 instantiation (pf_conv3_halo_e4m3_kernel, d.a_e4m3).  The sources are 64-channel segments of one e4m3
+// map, each k16 step becomes a k32 step (two per tap, wgmma.m64nBNk32.f32.e4m3.e4m3 with A from registers) and the
+// plain-output epilogue multiplies the accumulator by s_a[image] * s_w[column] before the bias.
+template <int CL, int BN, bool F8>
+__device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
   constexpr bool MC = CL > 1;
   constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1);
-  constexpr int kc = halo_kc(BN);                           // taps per B stage
-  constexpr int b_tile_bytes = BN * kBlockK * 2;
+  constexpr int EB = F8 ? 1 : 2;                            // bytes per operand element
+  constexpr int kRow = kBlockK * EB;                        // bytes of one pixel / weight row of a 64-channel chunk
+  constexpr int kc = halo_kc(BN, F8);                       // taps per B stage
+  constexpr int b_tile_bytes = BN * kRow;
   constexpr int b_stage_bytes = kc * b_tile_bytes;
-  constexpr int stages = halo_stages(BN);                   // B ring
+  constexpr int stages = halo_stages(BN, F8);               // B ring
+  constexpr int kSlot = halo_slot(F8);
+  constexpr int kKSteps = F8 ? 2 : kBlockK / 16;            // MMAs per tap
   extern __shared__ uint8_t smem_raw[];
   const GemmDesc& d = P.d;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_b = smem + kHaloSlots * kHaloSlot;
+  uint8_t* smem_b = smem + kHaloSlots * kSlot;
   uint8_t* xpose = smem_b + stages * b_stage_bytes;         // [kEpiWarps][2][2 KB] staging tiles, 1024-B aligned
   uint64_t* bars = reinterpret_cast<uint64_t*>(xpose + kEpiWarps * kStageWarp);
   uint64_t* a_full = bars;                                  // [kHaloSlots]
@@ -1149,6 +1193,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
         TileCoord c = decode_tile(d, it.tile(ti));
         tl.tile();
         int kbase = 0;                                       // first 64-wide K block of this source in the weights
+        int cbase = 0;                                       // F8: first 64-channel chunk of this source in the map
         for (int s = 0; s < d.num_src; ++s) {
           const int nch = d.chunks[s];
           for (int ch = 0; ch < nch; ++ch) {
@@ -1157,8 +1202,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
               mbar_wait(&a_empty[as], aph ^ 1);
               tl.add(1, tl_w);
               if (elect_one()) {
-                mbar_expect_tx(&a_full[as], kHaloBytes);
-                tma_load_4d(smem + as * kHaloSlot, &P.tmA[s], &a_full[as], ch * kBlockK, c.x0 - 1, c.y0 - 1, c.img);
+                mbar_expect_tx(&a_full[as], halo_bytes(F8));
+                tma_load_4d(smem + as * kSlot, &P.tmA[s], &a_full[as], (F8 ? cbase + ch : ch) * kBlockK, c.x0 - 1,
+                            c.y0 - 1, c.img);
               }
             }
             if (++as == kHaloSlots) { as = 0; aph ^= 1; }
@@ -1171,7 +1217,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
                 if (MC) {
                   constexpr int part_rows = BN / CL;
                   for (int j = 0; j < kc; ++j)
-                    tma_load_2d_mc(smem_b + bs * b_stage_bytes + j * b_tile_bytes + it.rank * part_rows * 128, &P.tmBh,
+                    tma_load_2d_mc(smem_b + bs * b_stage_bytes + j * b_tile_bytes + it.rank * part_rows * kRow, &P.tmBh,
                                    &b_full[bs], (kbase + (tap0 + j) * nch + ch) * kBlockK, c.n0 + it.rank * part_rows,
                                    kMask);
                 } else {
@@ -1184,6 +1230,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
             }
           }
           kbase += 9 * nch;
+          cbase += nch;
         }
       }
       tl.add(2, tl_start);
@@ -1199,7 +1246,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
             if (d.rs_h[s] != 0) {
               if ((turn & 1) == warp - kRsWarp0) {
                 mbar_wait(&a_empty[as], aph ^ 1);
-                halo_fill_bilinear(smem_u32(smem + as * kHaloSlot), d, s, ch, c, lane);
+                if constexpr (!F8) halo_fill_bilinear(smem_u32(smem + as * kSlot), d, s, ch, c, lane);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&a_full[as]);
               }
@@ -1216,9 +1263,9 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
     et.tm = &P.tmOut; et.stg_ptr = xpose + warp * kStageWarp; et.stg = smem_u32(et.stg_ptr); et.cur = 0;
     float* buf = reinterpret_cast<float*>(et.stg_ptr);
     const int arow = 16 * warp + (lane & 15);               // tile row this lane addresses for ldmatrix
-    const uint32_t a_off = static_cast<uint32_t>(((arow >> 3) * kHaloW + (arow & 7)) * 128);
+    const uint32_t a_off = static_cast<uint32_t>(((arow >> 3) * kHaloW + (arow & 7)) * kRow);
     float acc[BN / 2];
-    uint32_t fa[2][4][4];                                   // A fragments of two taps: one loads while the other is read
+    uint32_t fa[2][kKSteps][4];                             // A fragments of two taps: one loads while the other is read
     int as = 0; uint32_t aph = 0;
     int bs = 0; uint32_t bph = 0;
     int rbs = 0;                                            // oldest B stage not yet released
@@ -1234,7 +1281,7 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
           long long tl_w = tl.now();
           mbar_wait(&a_full[as], aph);
           tl.add(1, tl_w);
-          const uint32_t a_base = smem_u32(smem + as * kHaloSlot) + a_off;
+          const uint32_t a_base = smem_u32(smem + as * kSlot) + a_off;
           uint32_t sb = 0;
 #pragma unroll
           for (int tap = 0; tap < 9; ++tap) {
@@ -1246,11 +1293,15 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
               if (++bs == stages) { bs = 0; bph ^= 1; }
             }
             // fa[tap & 1] was last read by the group of tap - 2, retired by the wait below at tap - 1
-            halo_a_frags(a_base + static_cast<uint32_t>(((tap / 3) * kHaloW + tap % 3) * 128), lane, fa[tap & 1]);
-            const uint64_t bdesc = wgmma_desc_k128(sb + (tap % kc) * b_tile_bytes);
+            halo_a_frags(a_base + static_cast<uint32_t>(((tap / 3) * kHaloW + tap % 3) * kRow), lane, fa[tap & 1]);
+            const uint64_t bdesc = F8 ? wgmma_desc_k64(sb + (tap % kc) * b_tile_bytes)
+                                      : wgmma_desc_k128(sb + (tap % kc) * b_tile_bytes);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) Wgmma<BN>::rs(acc, fa[tap & 1][k], bdesc + 2 * k, accum | k);
+            for (int k = 0; k < kKSteps; ++k) {
+              if constexpr (F8) Wgmma8<BN>::rs(acc, fa[tap & 1][k], bdesc + 2 * k, accum | k);
+              else Wgmma<BN>::rs(acc, fa[tap & 1][k], bdesc + 2 * k, accum | k);
+            }
             wgmma_commit();
             accum = 1;
             wgmma_wait<1>();                                 // the group of tap - 1 is done
@@ -1271,7 +1322,8 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
       // plain bf16 outputs (the host sets tma_out for the whole launch): fragment layout, stmatrix staging, bulk
       // stores of {G ch, 8 px, 2 rows} boxes (TMA clips pixels past W / H, columns past the output and the phantom
       // img >= NB tile of a cluster); everything else row per thread
-      if (d.tma_out) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64>(d, et, acc, c, warp, lane);
+      if constexpr (F8) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, true>(d, et, acc, c, warp, lane);
+      else if (d.tma_out) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64>(d, et, acc, c, warp, lane);
       else epilogue_tile(d, c, acc, warp, lane, buf, nullptr);
       __syncwarp();
       tl.add(3, tl_epi);
@@ -1284,6 +1336,15 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __
   if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
 }
 
+template <int CL, int BN>
+__global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_kernel(const __grid_constant__ GemmKernelParams P) {
+  conv3_halo_body<CL, BN, false>(P);
+}
+template <int CL, int BN>
+__global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_kernel(const __grid_constant__ GemmKernelParams P) {
+  conv3_halo_body<CL, BN, true>(P);
+}
+
 
 // ------------------------------------------------------------------------------------------------------------
 // host side
@@ -1292,19 +1353,21 @@ static int g_sm_counts[kMaxDevices] = {0};
 
 using KernelFn = void (*)(GemmKernelParams);
 // pf_conv3_halo_kernel<CL, bn>, nullptr for a width without an instantiation
-template <int CL>
+template <int CL, bool F8>
 static KernelFn halo_kernel_cl(int bn) {
   switch (bn) {
-    case 32: return pf_conv3_halo_kernel<CL, 32>;
-    case 64: return pf_conv3_halo_kernel<CL, 64>;
-    case 128: return pf_conv3_halo_kernel<CL, 128>;
-    case 192: return pf_conv3_halo_kernel<CL, 192>;
+    case 32: return F8 ? pf_conv3_halo_e4m3_kernel<CL, 32> : pf_conv3_halo_kernel<CL, 32>;
+    case 64: return F8 ? pf_conv3_halo_e4m3_kernel<CL, 64> : pf_conv3_halo_kernel<CL, 64>;
+    case 128: return F8 ? pf_conv3_halo_e4m3_kernel<CL, 128> : pf_conv3_halo_kernel<CL, 128>;
+    case 192: return F8 ? pf_conv3_halo_e4m3_kernel<CL, 192> : pf_conv3_halo_kernel<CL, 192>;
     default: return nullptr;
   }
 }
-static KernelFn halo_kernel(int cl, int bn) {
-  return cl == 4 ? halo_kernel_cl<4>(bn) : (cl == 2 ? halo_kernel_cl<2>(bn) : halo_kernel_cl<1>(bn));
+template <bool F8>
+static KernelFn halo_kernel_t(int cl, int bn) {
+  return cl == 4 ? halo_kernel_cl<4, F8>(bn) : (cl == 2 ? halo_kernel_cl<2, F8>(bn) : halo_kernel_cl<1, F8>(bn));
 }
+static KernelFn halo_kernel(int cl, int bn, bool f8 = false) { return f8 ? halo_kernel_t<true>(cl, bn) : halo_kernel_t<false>(cl, bn); }
 // pf_gemm_kernel<MC, bn> for the widths of kGemmWidths, nullptr otherwise
 template <bool MC>
 static KernelFn gemm_kernel_mc(int bn) {
@@ -1332,9 +1395,10 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
         if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_kernel(mc, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (bool mc : {false, true})
       if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_pp_kernel(mc), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-    for (int cl : {1, 2, 4})
-      for (int bn : {32, 64, 128, 192})
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    for (bool f8 : {false, true})
+      for (int cl : {1, 2, 4})
+        for (int bn : {32, 64, 128, 192})
+          if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn, f8), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm kernels): %s", cudaGetErrorString(e));
     cudaDeviceGetAttribute(&g_sm_counts[dev], cudaDevAttrMultiProcessorCount, dev);
     attr_done[dev] = true;
@@ -1345,7 +1409,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     int ktrue = 0;
     for (int s = 0; s < d.num_src; ++s) ktrue += d.k_true[s];
     const int n_true = d.ps > 1 ? d.n_logical * d.ps * d.ps : d.N;
-    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? "conv3x3" : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : "linear")),
+    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? "conv3x3_e4m3" : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : "linear")),
               rows, d.taps, ktrue, n_true, d.act ? (d.act == PF_ACT_GELU ? " gelu" : (d.act == PF_ACT_RELU ? " relu" : " softplus")) : "",
               d.gamma ? " gamma" : (d.vt ? " vt" : ""), d.w2 ? " tail" : "");
   }
@@ -1364,11 +1428,12 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   if (P.total_tiles <= 0 || ks <= 0) return set_error("gemm: empty problem");
   int grid = P.total_tiles < g_sm_count ? P.total_tiles : g_sm_count;
   if (d.halo) {
-    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n);
+    const bool f8 = d.a_e4m3 != 0;
+    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n, f8);
     if (hk == nullptr) return set_error("conv3 halo: block_n %d (32, 64, 128 or 192)", d.block_n);
-    const int b_bytes = halo_kc(d.block_n) * d.block_n * kBlockK * 2;     // one weight stage
-    const int hstages = halo_stages(d.block_n);
-    size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * kHaloSlot + static_cast<size_t>(hstages) * b_bytes +
+    const int b_bytes = halo_kc(d.block_n, f8) * d.block_n * kBlockK * (f8 ? 1 : 2);     // one weight stage
+    const int hstages = halo_stages(d.block_n, f8);
+    size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * halo_slot(f8) + static_cast<size_t>(hstages) * b_bytes +
                    kEpiWarps * kStageWarp + kBarBytes;
     cudaError_t le;
     if (tmBh != nullptr) {
@@ -1385,22 +1450,23 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       at[1].val.programmaticStreamSerializationAllowed = 1;
       cfg.attrs = at;
       cfg.numAttrs = 1;
-      static int max_clusters[kMaxDevices][5] = {};
-      if (max_clusters[dev][cl] == 0) {
+      static int max_clusters[kMaxDevices][2][5] = {};
+      int (&mcl)[5] = max_clusters[dev][f8 ? 1 : 0];
+      if (mcl[cl] == 0) {
         cfg.gridDim = dim3(cl * (g_sm_count / cl));
         int n = 0;
         cudaError_t qe = cudaOccupancyMaxActiveClusters(&n, hk, &cfg);
         if (qe != cudaSuccess || n < 1) { cudaGetLastError(); n = g_sm_count / cl; }
-        max_clusters[dev][cl] = n < g_sm_count / cl ? n : g_sm_count / cl;
+        mcl[cl] = n < g_sm_count / cl ? n : g_sm_count / cl;
       }
-      const int clusters = groups < max_clusters[dev][cl] ? groups : max_clusters[dev][cl];
+      const int clusters = groups < mcl[cl] ? groups : mcl[cl];
       cfg.gridDim = dim3(cl * clusters);
       cfg.numAttrs = pdl_enabled() ? 2 : 1;
       le = cudaLaunchKernelEx(&cfg, hk, P);
     } else {
       le = launch_pdl(hk, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
     }
-    if (le != cudaSuccess) return set_error("pf_conv3_halo_kernel launch: %s", cudaGetErrorString(le));
+    if (le != cudaSuccess) return set_error("%s launch: %s", f8 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel", cudaGetErrorString(le));
   } else {
     if (d.pp && (d.block_n % kPpBN != 0 || d.num_src != 1 || d.a_mode != 0 || !d.tma_out))
       return set_error("gemm: the ping-pong kernel takes plain linear layers at block_n 128 / 256 (block_n %d)", d.block_n);
@@ -1431,7 +1497,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(e));
-  count_launch(d.halo ? "pf_conv3_halo_kernel" : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"));
+  count_launch(d.halo ? (d.a_e4m3 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel")
+                       : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"));
   return 0;
 }
 

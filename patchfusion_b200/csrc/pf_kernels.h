@@ -46,6 +46,11 @@ struct GemmDesc {
   int rs_any;
   int tma_out;           // pf_gemm_kernel epilogue through shared memory + TMA: 0 direct, 1 bf16 output, 2 fp32 output / residual stream
   int pp;                // plain linear layer through pf_gemm_pp_kernel (128 x 128 tiles, one per consumer warpgroup)
+  // E4M3 halo conv (pf_conv3_halo_kernel<CL, BN, true>): the sources are 64-channel-padded segments of ONE e4m3 map
+  // (pf_quantize_e4m3_tiles) read through tmA[0], the weights an e4m3 panel; acc * s_a[img] * s_w[col] before the bias
+  int a_e4m3;
+  const float* s_a;
+  const float* s_w;
 };
 
 int set_error(const char* fmt, ...);
@@ -107,6 +112,11 @@ int tmap_2d_f32(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows,
                 uint32_t box_rows);
 int tmap_3d_bf16(CUtensorMap* out, const void* ptr, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t ld1_elems,
                  uint64_t ld2_elems, uint32_t b0, uint32_t b1, uint32_t b2);
+// 8-bit elements (e4m3 operands): rows of 64 bytes use SWIZZLE_64B
+int tmap_2d_u8(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld_bytes, uint32_t box_cols,
+               uint32_t box_rows);
+int tmap_4d_nhwc_u8(CUtensorMap* out, const void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N, uint64_t ld_bytes,
+                    uint32_t box_c, uint32_t box_w, uint32_t box_h);
 int tmap_4d_nhwc_bf16(CUtensorMap* out, const void* ptr, uint64_t C, uint64_t W, uint64_t H, uint64_t N,
                       uint64_t ld_elems, uint32_t box_c, uint32_t box_w, uint32_t box_h);
 

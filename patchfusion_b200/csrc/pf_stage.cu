@@ -30,6 +30,7 @@ struct Ctx {
   void* stream;
   int err;
   pf_tap_fn tap; void* tap_user;
+  int n_e4m3;           // FP8 convs issued so far (names their debug taps)
 
   void* alloc(size_t bytes) {
     off = (off + 255) & ~static_cast<size_t>(255);
@@ -107,9 +108,56 @@ static void linear(Ctx& c, const pf_layer& L, const bf16* A, long long M, int co
   c.chk(pf_gemm(&d, c.stream));
 }
 
+// FP8 3x3 conv (a layer packed with pf_pack_weight_e4m3: fusion_precision 'fp8'): the sources are quantized with one
+// scale per tile (batch index) into one e4m3 map, which the E4M3 halo conv reads.  The map, the scales and the partial
+// maxima are bump-allocated here, so only FP8 layers change the workspace.
+static void conv_into_e4m3(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_ld,
+                           const GemmOpt& o) {
+  const int T = srcs[0]->B, H = srcs[0]->H, W = srcs[0]->W;
+  int kc = 0;
+  for (int i = 0; i < ns; ++i) kc += pad_to(srcs[i]->C, 64);
+  void* q = c.alloc(static_cast<size_t>(T) * H * W * kc);
+  float* s_a = static_cast<float*>(c.alloc(static_cast<size_t>(T) * 4));
+  float* part = static_cast<float*>(c.alloc(static_cast<size_t>(T) * PF_QUANT_PARTS * 4));
+  if (!c.live()) return;
+  if (out_ld % 8 || o.res1 || o.res2 || o.relu_copy || o.tail || o.gamma)
+    c.chk(set_error("FP8 conv: plain bf16 output only"));
+  const void* p[3] = {nullptr, nullptr, nullptr};
+  int32_t cc[3] = {0, 0, 0}, ld[3] = {0, 0, 0};
+  for (int i = 0; i < ns; ++i) { p[i] = srcs[i]->p; cc[i] = srcs[i]->C; ld[i] = srcs[i]->ld; }
+  if (c.live()) c.chk(pf_quantize_e4m3_tiles(ns, p, cc, ld, T, H, W, part, q, s_a, c.stream));
+  if (!c.live()) return;
+  pf_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.num_src = ns; d.a_mode = 1;
+  d.a_ptr[0] = q;
+  for (int i = 0; i < ns; ++i) { d.a_c[i] = pad_to(srcs[i]->C, 8); d.a_ld[i] = kc; }
+  d.NB = T; d.H = H; d.W = W;
+  gemm_desc_common(d, L, o, out, 0, out_ld);
+  d.w_ptr = L.w8;
+  d.a_e4m3 = 1; d.s_a = s_a; d.s_w = L.w_scale;
+  c.chk(pf_gemm(&d, c.stream));
+  // debug taps "e4m3.<k>.src<i>.<H>x<W>" / "e4m3.<k>.out.<H>x<W>": the k-th FP8 conv's bf16 inputs and its output, so a
+  // test can check each conv against a reference on exactly the input the kernel saw
+  if (c.tap != nullptr && c.live()) {
+    char nm[48];
+    for (int i = 0; i < ns; ++i) {
+      snprintf(nm, sizeof(nm), "e4m3.%d.src%d.%dx%d", c.n_e4m3, i, H, W);
+      c.tap_out(nm, srcs[i]->p, 0, srcs[i]->rows(), srcs[i]->C, srcs[i]->ld);
+    }
+    snprintf(nm, sizeof(nm), "e4m3.%d.out.%dx%d", c.n_e4m3, H, W);
+    c.tap_out(nm, out, 0, static_cast<long long>(T) * H * W, L.N, out_ld);
+  }
+  ++c.n_e4m3;
+}
+
 // 3x3 / 1x1 conv over up to three channel-concatenated NHWC sources
 static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_f32, int out_ld,
                       const GemmOpt& o = GemmOpt()) {
+  if (L.w_scale != nullptr && L.taps == 9 && !out_f32) {
+    conv_into_e4m3(c, L, srcs, ns, out, out_ld, o);
+    return;
+  }
   if (!c.live()) return;
   pf_gemm_desc d;
   memset(&d, 0, sizeof(d));
@@ -135,6 +183,11 @@ static Map conv_resampled(Ctx& c, const pf_layer& L, const Map* const* srcs, int
     return out;
   }
   if (!c.live()) return out;
+  // an FP8 layer reads its bf16 panel here: the resample is produced inside the conv, there is no input to quantize
+  if (L.w == nullptr) {
+    c.chk(set_error("fused-resample conv: layer has no bf16 panel"));
+    return out;
+  }
   pf_gemm_desc d;
   memset(&d, 0, sizeof(d));
   d.num_src = ns; d.a_mode = 1;
@@ -499,7 +552,7 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
 static Ctx make_ctx(void* ws, size_t bytes, bool dry, void* stream, pf_tap_fn tap, void* user) {
   Ctx c;
   c.base = static_cast<uint8_t*>(ws); c.cap = bytes; c.off = 0; c.dry = dry; c.stream = stream; c.err = 0;
-  c.tap = tap; c.tap_user = user;
+  c.tap = tap; c.tap_user = user; c.n_e4m3 = 0;
   return c;
 }
 

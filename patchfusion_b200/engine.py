@@ -23,7 +23,7 @@ import torch.nn.functional as F
 
 from . import lib, ops
 from .ops import ACT_GELU, ACT_NONE, ACT_RELU, ACT_SOFTPLUS, call, pad_to, stream_ptr
-from .params import WINDOW, branch_hparams, guided_fusion_hparams, normed_attractors, _get
+from .params import WINDOW, branch_hparams, fusion_precision, guided_fusion_hparams, normed_attractors, _get
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -89,14 +89,20 @@ class Engine:
     def _w(self, k):
         return self.sd[k]
 
-    def _conv(self, name, src_c=None, bias=True):
+    def _conv(self, name, src_c=None, bias=True, fp8=None):
+        """fp8: None packs bf16; 'only' / 'keep_bf16' packs e4m3 (pack_weight_e4m3), the latter with the bf16 panel
+        too (a conv that may read its input through the fused resample)."""
         b = self._w(name + '.bias') if bias and (name + '.bias') in self.sd else None
+        if fp8:
+            return ops.pack_weight_e4m3(self._w(name + '.weight'), b, src_c=src_c, keep_bf16=fp8 == 'keep_bf16')
         return ops.pack_weight(self._w(name + '.weight'), b, src_c=src_c)
 
-    def _conv_bn(self, conv, bn):
+    def _conv_bn(self, conv, bn, fp8=None):
         g, b = self._w(bn + '.weight'), self._w(bn + '.bias')
         m, v = self._w(bn + '.running_mean'), self._w(bn + '.running_var')
         scale = g / torch.sqrt(v + 1e-5)
+        if fp8:
+            return ops.pack_weight_e4m3(self._w(conv + '.weight'), None, scale=scale, shift=b - m * scale)
         return ops.pack_weight(self._w(conv + '.weight'), None, scale=scale, shift=b - m * scale)
 
     def _f32(self, k):
@@ -187,21 +193,26 @@ class Engine:
         hp = self.hp['fine']
         C = hp['features']
         Wd = {}
+        # fusion_precision 'fp8': the U-Net's 3x3 convs get e4m3 panels; the convs whose input can come through the
+        # fused resample (up*.0, cv*.0) keep their bf16 panel for that path too.  fusion_conv_list, G2L and the head
+        # stay bf16.
+        f8 = 'only' if fusion_precision(self.cfg) == 'fp8' else None
+        f8rs = 'keep_bf16' if f8 else None
         for i in range(5):      # level 5's fused map is dead in the U-Net (guided_fusion_model.py:198)
             Wd['fc%d' % i] = self._conv('fusion_conv_list.%d' % i, src_c=[C, C])
         g = 'guided_fusion.'
         ic = self.gf['in_channels']
-        Wd['inc.0'] = self._conv_bn(g + 'inc.double_conv.0', g + 'inc.double_conv.1')
-        Wd['inc.1'] = self._conv_bn(g + 'inc.double_conv.3', g + 'inc.double_conv.4')
+        Wd['inc.0'] = self._conv_bn(g + 'inc.double_conv.0', g + 'inc.double_conv.1', fp8=f8)
+        Wd['inc.1'] = self._conv_bn(g + 'inc.double_conv.3', g + 'inc.double_conv.4', fp8=f8)
         for i in range(5):
             p = g + 'down_conv_list.%d.maxpool_conv.1.double_conv.' % i
-            Wd['down%d.0' % i] = self._conv_bn(p + '0', p + '1')
-            Wd['down%d.1' % i] = self._conv_bn(p + '3', p + '4')
+            Wd['down%d.0' % i] = self._conv_bn(p + '0', p + '1', fp8=f8)
+            Wd['down%d.1' % i] = self._conv_bn(p + '3', p + '4', fp8=f8)
         inv = ic[::-1]
         for i in range(1, 6):
             p = g + 'up_conv_list.%d.conv.double_conv.' % (i - 1)
-            Wd['up%d.0' % i] = self._conv(p + '0', src_c=[inv[i], inv[i - 1], inv[i - 1]])
-            Wd['up%d.1' % i] = self._conv(p + '2')
+            Wd['up%d.0' % i] = self._conv(p + '0', src_c=[inv[i], inv[i - 1], inv[i - 1]], fp8=f8rs)
+            Wd['up%d.1' % i] = self._conv(p + '2', fp8=f8)
         depth, heads = self.gf['depth'][::-1], self.gf['num_heads'][::-1]
         for i in range(6):
             c, p = inv[i], g + 'g2l_list.%d.' % i
@@ -220,8 +231,8 @@ class Engine:
                     fc2=ops.pack_weight(self._w(q + 'mlp.fc2.weight'), self._w(q + 'mlp.fc2.bias'))))
             Wd['g2l%d' % i] = L
             p = g + 'convs.%d.double_conv.' % i
-            Wd['cv%d.0' % i] = self._conv(p + '0', src_c=[c, c])
-            Wd['cv%d.1' % i] = self._conv(p + '2')
+            Wd['cv%d.0' % i] = self._conv(p + '0', src_c=[c, c], fp8=f8rs)
+            Wd['cv%d.1' % i] = self._conv(p + '2', fp8=f8)
         Wd['head'] = self._pack_head('', C, self.hp['coarse'], drop_rel=True)
         return Wd
 

@@ -15,6 +15,7 @@ LIB_PATH = os.path.join(HERE, os.environ.get('PF_B200_LIBNAME', 'libpf_b200.so')
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_SOFTPLUS = 0, 1, 2, 3
 # include/pf_b200.h PF_BINS_* (pf_head.bin_centers_type) and PF_SEED_* (pf_seed_bins flags)
 BINS_TYPES = {'softplus': 0, 'normed': 1, 'hybrid1': 2, 'hybrid2': 3}
+QUANT_PARTS = 32    # PF_QUANT_PARTS: partial maxima per tile of pf_quantize_e4m3_tiles
 SEED_NORMED, SEED_TO_UNIT = 1, 2
 OPT_TMA_EPILOGUE, OPT_HALO_MULTICAST, OPT_GEMM_MULTICAST, OPT_FUSED_RESAMPLE, OPT_PDL, OPT_RESIZE_SEPARABLE = 0, 1, 2, 3, 4, 5
 
@@ -42,6 +43,7 @@ class GemmDesc(C.Structure):
         ('w2', C.c_void_p), ('b2', C.c_void_p), ('n2', C.c_int32), ('act2', C.c_int32), ('skip_main', C.c_int32),
         ('out3', C.c_void_p), ('out3_ld', C.c_int32),
         ('rs_h', C.c_int32 * 3), ('rs_w', C.c_int32 * 3),
+        ('a_e4m3', C.c_int32), ('s_a', C.c_void_p), ('s_w', C.c_void_p),
     ]
 
 
@@ -61,6 +63,9 @@ SIGNATURES = {
     'pf_gemm': [C.POINTER(GemmDesc), _p],
     'pf_pack_weight': [_p, _i, _i, _i, C.POINTER(C.c_int32), _i, _p, _p, _p],
     'pf_pack_weight_convT': [_p, _i, _i, _i, _p, _p],
+    'pf_pack_weight_e4m3': [_p, _i, _i, _i, C.POINTER(C.c_int32), _i, _p, _p, _p, _p],
+    'pf_quantize_e4m3_tiles': [_i, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _i, _i, _p,
+                               _p, _p, _p],
     'pf_layernorm': [_p, _i, _p, _p, _f, _i, _i, _p, _i, _p],
     'pf_layernorm_grouped': [_p, _i, _p, _p, _f, _i, _i, _i, _i, _i, _p, _i, _p],
     'pf_attention': [_p, _i, _p, _i, _i, _i, _i, _f, _p, _i, _p],

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .params import ParamTree, _get, state_layout, synthetic_state_dict, relative_position_index
+from .params import ParamTree, _get, fusion_precision, state_layout, synthetic_state_dict, relative_position_index
 
 try:
     from huggingface_hub import PyTorchModelHubMixin
@@ -506,6 +506,7 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         self.patch_process_shape = config.patch_process_shape
         self.tile_cfg = self.prepare_tile_cfg(config.image_raw_shape, config.patch_split_num)
         self.coarse_branch_cfg = config.coarse_branch
+        self.fusion_precision = fusion_precision(config)     # ValueError on anything but 'bf16' / 'fp8'
         for br in (config.coarse_branch, config.fine_branch):
             if br.type not in ('ZoeDepth', 'DA-ZoeDepth'):
                 raise NotImplementedError

@@ -16,7 +16,10 @@ def pad_to(n, m):
 
 
 class PackedWeight:
-    """bf16 K-major weight panel for pf_gemm + fp32 bias."""
+    """bf16 K-major weight panel for pf_gemm + fp32 bias.  An FP8 layer (pack_weight_e4m3) also has an e4m3 panel `w8`
+    [N_pad, Ktot] (uint8 storage) and its per-output-channel scales `w_scale` [N]; its bf16 `w` may be None."""
+    w8 = None
+    w_scale = None
 
     def __init__(self, w, bias, N, src_c, taps, ps=1, ps_cout=0):
         self.w, self.bias, self.N, self.src_c, self.taps = w, bias, N, list(src_c), taps
@@ -61,6 +64,70 @@ def pack_weight(weight, bias=None, src_c=None, scale=None, shift=None):
         if shift is not None:
             b += shift.float()
     return PackedWeight(dst, b, N, src_c, taps)
+
+
+def pack_weight_e4m3(weight, bias=None, src_c=None, scale=None, shift=None, keep_bf16=False):
+    """pack_weight's panel as e4m3 with one fp32 scale per output channel (pf_pack_weight_e4m3; the rounding rule is
+    in include/pf_b200.h).  keep_bf16: also keep the bf16 panel (a conv that may run through the fused resample)."""
+    pw = pack_weight(weight, bias, src_c=src_c, scale=scale, shift=shift)
+    weight = weight.float().contiguous()
+    w8 = torch.empty(pw.w.shape, dtype=torch.uint8, device=weight.device)
+    s_w = torch.empty(pw.N, dtype=torch.float32, device=weight.device)
+    sc = (C.c_int32 * 3)(*(pw.src_c + [0] * (3 - len(pw.src_c))))
+    scale_t = scale.float().contiguous() if scale is not None else None
+    call('pf_pack_weight_e4m3', weight, pw.N, pw.w.shape[0], len(pw.src_c), sc, pw.taps, scale_t, w8, s_w, stream_ptr())
+    pw.w8, pw.w_scale = w8, s_w
+    if not keep_bf16:
+        pw.w = None
+    return pw
+
+
+def quantize_e4m3_tiles(srcs, src_c=None, out=None, s_a=None):
+    """srcs: bf16 NHWC maps [T,H,W,ld_i] (logical channels src_c[i], default the last dim).  Returns (q, s_a): the
+    e4m3 map [T,H,W,Kc] (uint8 storage, sources back to back, each padded to 64 channels) and the fp32 tile scales [T]
+    (pf_quantize_e4m3_tiles)."""
+    T, H, W = srcs[0].shape[:3]
+    cs = [s_.shape[-1] for s_ in srcs] if src_c is None else list(src_c)
+    kc = sum(pad_to(c, 64) for c in cs)
+    dev = srcs[0].device
+    for s_ in srcs:
+        assert s_.dtype == torch.bfloat16 and s_.is_contiguous() and tuple(s_.shape[:3]) == (T, H, W)
+    if out is None:
+        out = torch.empty((T, H, W, kc), dtype=torch.uint8, device=dev)
+    if s_a is None:
+        s_a = torch.empty(T, dtype=torch.float32, device=dev)
+    assert out.dtype == torch.uint8 and tuple(out.shape) == (T, H, W, kc) and out.is_contiguous()
+    part = torch.empty(T * lib.QUANT_PARTS, dtype=torch.float32, device=dev)
+    n = len(srcs)
+    ptrs = (C.c_void_p * 3)(*([s_.data_ptr() for s_ in srcs] + [None] * (3 - n)))
+    cc = (C.c_int32 * 3)(*(cs + [0] * (3 - n)))
+    ld = (C.c_int32 * 3)(*([s_.shape[-1] for s_ in srcs] + [0] * (3 - n)))
+    call('pf_quantize_e4m3_tiles', n, ptrs, cc, ld, T, H, W, part, out, s_a, stream_ptr())
+    return out, s_a
+
+
+def conv3_e4m3(pw, q, s_a, out, act=ACT_NONE, block_n=0):
+    """The E4M3 halo conv: q / s_a from quantize_e4m3_tiles over sources with pw.src_c channels, pw from
+    pack_weight_e4m3, out bf16 NHWC [T,H,W,ld]."""
+    T, H, W, kc = q.shape
+    assert q.dtype == torch.uint8 and kc == sum(pad_to(c, 64) for c in pw.src_c) and pw.taps == 9
+    d = GemmDesc()
+    d.num_src = len(pw.src_c)
+    d.taps = 9
+    d.a_mode = 1
+    d.a_ptr[0] = q.data_ptr()
+    for i, c in enumerate(pw.src_c):
+        d.a_c[i], d.a_ld[i] = pad_to(c, 8), kc
+    d.NB, d.H, d.W = T, H, W
+    d.w_ptr = pw.w8.data_ptr()
+    d.N, d.Ktot, d.block_n = pw.N, pw.Ktot, block_n
+    d.bias = pw.bias.data_ptr() if pw.bias is not None else None
+    d.act = act
+    assert out.dtype == torch.bfloat16 and out.is_contiguous()
+    d.out, d.out_ld = out.data_ptr(), out.shape[-1]
+    d.a_e4m3, d.s_a, d.s_w = 1, s_a.data_ptr(), pw.w_scale.data_ptr()
+    call('pf_gemm', C.byref(d), stream_ptr())
+    return d
 
 
 def pack_weight_convT(weight, bias, k):

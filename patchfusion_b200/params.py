@@ -37,6 +37,19 @@ def _get(cfg, key, default=None):
     return getattr(cfg, key, default)
 
 
+FUSION_PRECISIONS = ('bf16', 'fp8')
+
+
+def fusion_precision(config):
+    """Top-level `fusion_precision`: what the Guided-Fusion U-Net's 3x3 convs (inc, down_conv_list, up_conv_list, convs)
+    compute in.  'bf16' (default) is the path every other layer takes; 'fp8' runs them on E4M3 operands with one
+    scale per tile and input and one per output channel (include/pf_b200.h, DESIGN.md section 7)."""
+    p = _get(config, 'fusion_precision', 'bf16')
+    if p not in FUSION_PRECISIONS:
+        raise ValueError("fusion_precision should be one of 'bf16', 'fp8'")
+    return p
+
+
 def branch_hparams(branch_cfg):
     enc = _get(branch_cfg, 'midas_model_type')
     if enc not in ENCODERS:

@@ -12,7 +12,7 @@ i32, f32, vp = C.c_int32, C.c_float, C.c_void_p
 
 class PfLayer(C.Structure):
     _fields_ = [('w', vp), ('bias', vp), ('N', i32), ('Ktot', i32), ('taps', i32), ('num_src', i32), ('src_c', i32 * 3),
-                ('ps', i32), ('ps_cout', i32), ('w2', vp), ('b2', vp), ('n2', i32)]
+                ('ps', i32), ('ps_cout', i32), ('w2', vp), ('b2', vp), ('n2', i32), ('w8', vp), ('w_scale', vp)]
 
 
 class PfVitBlock(C.Structure):
@@ -102,9 +102,12 @@ def _check(rc, what):
 
 
 def layer(pw, tail=None):
-    """PackedWeight (+ optional fp32 trailing layer (w2 [n2, N], b2)) -> PfLayer.  The caller keeps the tensors alive."""
+    """PackedWeight (+ optional fp32 trailing layer (w2 [n2, N], b2)) -> PfLayer.  The caller keeps the tensors alive.
+    An FP8 layer (PackedWeight.w8 set) carries its e4m3 panel and scales, and its bf16 panel only when it has one."""
     L = PfLayer()
-    L.w = pw.w.data_ptr()
+    L.w = pw.w.data_ptr() if pw.w is not None else None
+    if getattr(pw, 'w8', None) is not None:
+        L.w8, L.w_scale = pw.w8.data_ptr(), pw.w_scale.data_ptr()
     L.bias = pw.bias.data_ptr() if pw.bias is not None else None
     L.N, L.Ktot, L.taps = pw.N, pw.Ktot, pw.taps
     L.num_src = len(pw.src_c)
