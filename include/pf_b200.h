@@ -118,6 +118,18 @@ typedef struct pf_gemm_desc {
   int32_t a_e4m3;
   const float* s_a;
   const float* s_w;
+  /* Static input scale (fusion_precision 'fp8_static'; a_e4m3 != 0): a_static != 0 replaces s_a[img] by the one value
+   * a_scale (amax / 448 of the conv's calibrated input amax) for the whole launch: act(fl(acc * fl(a_scale * s_w[n])) +
+   * bias[n]).  s_a may then be NULL.
+   * E4M3 output (out_e4m3 != 0; needs a_static): the activated fp32 value v is written as q = e4m3_rn(sat(v * out_ratio))
+   * (the consumer's r = 448 / amax, pf_quantize_e4m3_static's rule) into `out`, an e4m3 NHWC map [NB, H, W, out_ld
+   * bytes] whose columns N .. 64 ceil(N / 64) - 1 are written as zero: the operand map of a one-source E4M3 conv.
+   * out_ld a multiple of 16 >= 64 ceil(N / 64), out_col0 0, `out` 16-byte aligned, a plain output (no residual, second
+   * output, trailing layer or fp32), and block_n 32 only when N <= 32. */
+  int32_t a_static;
+  float a_scale;
+  int32_t out_e4m3;
+  float out_ratio;
 } pf_gemm_desc;
 
 int pf_gemm(pf_gemm_desc* desc, void* stream);
@@ -156,6 +168,15 @@ int pf_pack_weight_e4m3(const float* w, int32_t N, int32_t N_pad, int32_t num_sr
 #define PF_QUANT_PARTS 32
 int pf_quantize_e4m3_tiles(int32_t num_src, const void* const* src, const int32_t* src_c, const int32_t* src_ld,
                            int32_t T, int32_t H, int32_t W, float* partial, void* out, float* s_a, void* stream);
+/* ---- Static E4M3 activations (fusion_precision = 'fp8_static'): one calibrated amax per conv input ---------------
+ *   r = 448 / amax (one IEEE fp32 division), or 0 when amax == 0;   scale = amax / 448
+ *   q = e4m3_rn(sat(v * r))   cvt.rn.satfinite: |v * r| beyond 448 (the input may exceed the calibrated amax) gives
+ *                             +-448, an infinity too; NaN stays NaN; the sign of zero is kept
+ * pf_quantize_e4m3_tiles' sources and output map (each source padded to 64 channels, pad channels zero) at the given
+ * ratio r for every tile: ONE launch that reads each bf16 source once, no amax pass.  A tile's bytes depend on the tile
+ * only. */
+int pf_quantize_e4m3_static(int32_t num_src, const void* const* src, const int32_t* src_c, const int32_t* src_ld,
+                            int32_t T, int32_t H, int32_t W, float ratio, void* out, void* stream);
 
 /* ---- ViT pieces --------------------------------------------------------------------------------------------- */
 /* LayerNorm over the last dim, fp32 in -> bf16 out (dinov2/layers/block.py:84,87; vision_transformer.py:311;
@@ -381,6 +402,11 @@ typedef struct pf_layer {
    * (PF_OPT_FUSED_RESAMPLE), which has no materialised input to quantize and stays bf16. */
   const void* w8;
   const float* w_scale;
+  /* fusion_precision 'fp8_static': a HOST pointer to the calibrated amax of the conv's input (NULL: per-tile scales as
+   * above).  The stage then quantizes the input with pf_quantize_e4m3_static at r = 448 / amax and runs the conv with the
+   * static scale amax / 448; the first conv of a U-Net DoubleConv whose second conv is static too writes the second's
+   * e4m3 operand map directly (pf_gemm_desc.out_e4m3).  Read when the stage is issued. */
+  const float* a_amax;
 } pf_layer;
 
 typedef struct pf_vit_block {             /* dinov2/layers/block.py:82-107 */

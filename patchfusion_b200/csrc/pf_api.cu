@@ -399,6 +399,35 @@ __global__ void quant_write_kernel(QuantSrc q, long long hw, const float* __rest
   }
 }
 
+// pf_quantize_e4m3_static: quant_write_kernel's map at one ratio for every tile (e4m3x2's cvt.rn.satfinite saturates
+// |v * r| > 448 to +-448); one pass over the sources, 8 output channels per thread
+__global__ void quant_static_kernel(QuantSrc q, long long pixels, float r, uint8_t* __restrict__ out) {
+  const int g = q.kc / 8;
+  const long long items = pixels * g;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < items;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long px = i / g;
+    const int k = 8 * static_cast<int>(i - px * g);
+    int s = q.ns - 1;
+    while (s > 0 && k < q.koff[s]) --s;
+    const int c = k - q.koff[s];
+    uint32_t lo = 0, hi = 0;
+    if (c < q.c[s]) {
+      const uint4 u = __ldg(reinterpret_cast<const uint4*>(q.p[s] + px * q.ld[s] + c));
+      const uint32_t wv[4] = {u.x, u.y, u.z, u.w};
+      float v[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const float x = __uint_as_float(e & 1 ? (wv[e >> 1] & 0xffff0000u) : (wv[e >> 1] << 16));
+        v[e] = c + e < q.c[s] ? __fmul_rn(x, r) : 0.f;
+      }
+      lo = e4m3x2(v[0], v[1]) | (e4m3x2(v[2], v[3]) << 16);
+      hi = e4m3x2(v[4], v[5]) | (e4m3x2(v[6], v[7]) << 16);
+    }
+    *reinterpret_cast<uint2*>(out + px * q.kc + k) = make_uint2(lo, hi);
+  }
+}
+
 }  // namespace pf
 
 using namespace pf;
@@ -496,6 +525,33 @@ int pf_quantize_e4m3_tiles(int32_t num_src, const void* const* src, const int32_
   return check_launch("quant_write_kernel");
 }
 
+int pf_quantize_e4m3_static(int32_t num_src, const void* const* src, const int32_t* src_c, const int32_t* src_ld,
+                            int32_t T, int32_t H, int32_t W, float ratio, void* out, void* stream) {
+  if (num_src < 1 || num_src > 3 || !src || !src_c || !src_ld || T < 1 || H < 1 || W < 1 || !out || !(ratio >= 0.f))
+    return set_error("pf_quantize_e4m3_static: bad arguments");
+  QuantSrc q;
+  memset(&q, 0, sizeof(q));
+  q.ns = num_src;
+  for (int s = 0; s < num_src; ++s) {
+    q.p[s] = static_cast<const __nv_bfloat16*>(src[s]);
+    q.c[s] = src_c[s]; q.ld[s] = src_ld[s]; q.koff[s] = q.kc;
+    if (!src[s] || src_c[s] < 1 || src_ld[s] < (src_c[s] + 7) / 8 * 8 || src_ld[s] % 8 || reinterpret_cast<uintptr_t>(src[s]) & 15)
+      return set_error("pf_quantize_e4m3_static: source %d: channels %d, ld %d (a multiple of 8 covering them), 16-byte aligned",
+                       s, src_c[s], src_ld[s]);
+    q.kc += (src_c[s] + 63) / 64 * 64;
+  }
+  if (reinterpret_cast<uintptr_t>(out) & 7) return set_error("pf_quantize_e4m3_static: output not 8-byte aligned");
+  const long long pixels = static_cast<long long>(T) * H * W;
+  const long long items = pixels * (q.kc / 8);
+  long long bx = (items + 255) / 256;
+  const long long cap = 8LL * sm_count();
+  if (bx > cap) bx = cap;
+  note_work(0.0, "quantize e4m3 static T%d %dx%d K%d", T, H, W, q.kc);
+  quant_static_kernel<<<static_cast<unsigned>(bx), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      q, pixels, ratio, static_cast<uint8_t*>(out));
+  return check_launch("quant_static_kernel");
+}
+
 int pf_pack_weight_convT(const float* w, int32_t Cin, int32_t Cout, int32_t k, void* dst, void* stream) {
   int Kp = (Cin + 63) / 64 * 64;
   long long total = static_cast<long long>(k) * k * ((Cout + 31) / 32 * 32) * Kp;
@@ -524,9 +580,18 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   if (u->N <= 0) return set_error("pf_gemm: N %d", u->N);
   if (u->out_ld % 8 || u->out_col0 % 8) return set_error("pf_gemm: out_ld/out_col0 must be multiples of 8");
   const bool e4m3 = u->a_e4m3 != 0;
+  const bool a_static = e4m3 && u->a_static != 0;
   if (e4m3 && (u->a_mode != 1 || u->taps != 9 || u->bh != 0 || u->bw != 0 || getenv("PF_B200_NO_HALO") != nullptr ||
-               u->rs_h[0] || u->rs_h[1] || u->rs_h[2] || !u->s_a || !u->s_w))
+               u->rs_h[0] || u->rs_h[1] || u->rs_h[2] || (!u->s_a && !a_static) || !u->s_w))
     return set_error("pf_gemm: e4m3 operands take the 3x3 halo-tile conv with materialised sources and s_a / s_w");
+  if ((u->a_static && !e4m3) || (u->out_e4m3 && !a_static))
+    return set_error("pf_gemm: a static input scale needs e4m3 operands, an e4m3 output a static input scale");
+  const bool out8 = u->out_e4m3 != 0;
+  const int n_pad64 = (u->N + 63) / 64 * 64;
+  if (out8 && (u->out_f32 || u->gamma || u->res1 || u->res2 || u->out2 || u->w2 || u->vt || u->ps > 1 || u->out_col0 ||
+               u->out_ld % 16 || u->out_ld < n_pad64 || reinterpret_cast<uintptr_t>(u->out) % 16 || !(u->out_ratio >= 0.f)))
+    return set_error("pf_gemm: an e4m3 output is a plain map of 64 ceil(N / 64) <= out_ld (a multiple of 16) byte rows, "
+                     "16-byte aligned, with out_ratio >= 0");
   GemmDesc d;
   memset(&d, 0, sizeof(d));
   d.num_src = u->num_src; d.a_mode = u->a_mode; d.taps = u->taps;
@@ -638,11 +703,23 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
         if (n_pad % w == 0) bn = w;
     }
   }
+  // An e4m3 output is stored in 64-byte column groups: a 32-column n-tile would share its group with the next one.  So
+  // such a conv takes 64-column n-tiles even where the panel's n_pad rows are a multiple of 32 only (N = 160 in the
+  // vits U-Net): its weight maps then end at n_pad rows and the copy engine zero-fills the rows past them.
+  uint64_t b_rows = 0;
+  if (out8 && bn == 32 && u->N > 32) {
+    if (u->block_n != 0) return set_error("pf_gemm: an e4m3 output needs block_n >= 64 when N > 32 (N %d)", u->N);
+    bn = 64;
+    b_rows = static_cast<uint64_t>(n_pad);
+  }
   d.block_n = bn; d.N = u->N; d.n_tiles = (u->N + bn - 1) / bn;
   u->block_n = bn; u->n_tiles = d.n_tiles;
+  if (b_rows == 0) b_rows = static_cast<uint64_t>(d.n_tiles) * bn;
   if (e4m3) {
-    if (tmap_2d_u8(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) return 1;
+    if (tmap_2d_u8(&tmB, u->w_ptr, u->Ktot, b_rows, u->Ktot, 64, bn)) return 1;
     d.a_e4m3 = 1; d.s_a = u->s_a; d.s_w = u->s_w;
+    d.a_static = a_static ? 1 : 0; d.a_scale = u->a_scale;
+    d.out_e4m3 = out8 ? 1 : 0; d.out_ratio = u->out_ratio;
   } else if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) {
     return 1;
   }
@@ -691,7 +768,7 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   d.halo_cl = halo ? cl : 1;
   const bool mc = cl > 1;
   CUtensorMap tmBh;
-  if (mc && (e4m3 ? tmap_2d_u8(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)
+  if (mc && (e4m3 ? tmap_2d_u8(&tmBh, u->w_ptr, u->Ktot, b_rows, u->Ktot, 64, bn / cl)
                   : tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn / cl)))
     return 1;
   // Epilogue through shared memory + TMA: plain bf16 outputs in 64-column groups (32-column groups in the halo kernel at
@@ -705,7 +782,12 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   // the staged zeros of columns N .. written over what the caller keeps there, so such outputs take the direct stores.
   const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;
   const bool ends16 = ocols % (d.out_f32 ? 4 : 8) == 0;
-  if (!no_tma_epi && !(halo && any_rs) && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
+  if (out8) {
+    // the q8 kernel's e4m3 epilogue: {64 bytes, 8 px, 2 rows} boxes of a map N rounded up to 64 columns wide, so the
+    // stores write the pad columns (as zero) too
+    if (!no_tma_epi && tmap_4d_nhwc_u8(&tmOut, u->out, n_pad64, u->W, u->H, u->NB, u->out_ld, 64, 8, 2)) return 1;
+    d.tma_out = no_tma_epi ? 0 : 1;
+  } else if (!no_tma_epi && !(halo && any_rs) && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
     // each consumer warp stores its 16 rows in whole column groups (bf16) / 32-column chunks (fp32)
     const uint32_t group = halo && bn == 32 ? 32 : 64;
     if (!d.out_f32 && bn % group == 0 && reinterpret_cast<uintptr_t>(u->out) % 16 == 0) {

@@ -460,12 +460,14 @@ __device__ __forceinline__ void epi_dequant(const GemmDesc& d, float (&v)[16], i
     v[4 * j + 2] = __fmul_rn(v[4 * j + 2], kx); v[4 * j + 3] = __fmul_rn(v[4 * j + 3], ky);
   }
 }
-template <int G, int S, bool SC = false>
+// SC = 2 (the static-scale instantiation): the one scale d.a_scale of the launch instead of s_a[img].
+template <int G, int S, int SC = 0>
 __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                        const TileCoord& c, int warp, int lane) {
   static_assert(G == 64 || G == 32, "group width");
   float sa = 0.f;
-  if constexpr (SC) sa = c.img < d.NB ? __ldg(d.s_a + c.img) : 0.f;   // img >= NB: a cluster's phantom tile
+  if constexpr (SC == 1) sa = c.img < d.NB ? __ldg(d.s_a + c.img) : 0.f;   // img >= NB: a cluster's phantom tile
+  if constexpr (SC == 2) sa = d.a_scale;
   const int oct = lane >> 4;
   const uint32_t lane_off = (lane & 15) * (2 * G);
   const int swz = G == 64 ? (lane & 7) : ((lane >> 1) & 3);
@@ -477,7 +479,7 @@ __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma
     for (int h = 0; h < G / 32; ++h) {
       float v[16];
       acc_chunk(G / 32 * g + h, acc, v);
-      if constexpr (SC) epi_dequant(d, v, lcol + 32 * h + 2 * (lane & 3), sa);
+      if constexpr (SC != 0) epi_dequant(d, v, lcol + 32 * h + 2 * (lane & 3), sa);
       epi_frag(d, v, lcol + 32 * h + 2 * (lane & 3), false);
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
@@ -491,6 +493,66 @@ __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma
     __syncwarp();
     if (lane == 0) {
       epi_tma_store(d, e, e.stg_ptr + tile, c, warp, d.out_col0 + lcol);
+      bulk_commit();
+    }
+  }
+}
+
+// e4m3 output (the static-scale halo conv with d.out_e4m3): the dequantized, biased and activated fp32 value v of
+// each element is quantized straight to e4m3_rn(sat(v * out_ratio)), never through bf16, and stored as the operand map
+// of the next E4M3 conv: groups of 64 columns = 64-byte row segments (SWIZZLE_64B: 16-byte piece j of row r at
+// j ^ ((r >> 1) & 3)), one {64 B, 8 px, 2 rows} bulk store per warp and group.  A thread's fragment gives two adjacent
+// columns per row and octet, so it writes them as one 16-bit e4m3x2 at byte 32h + 8j + 2 (lane % 4) of rows lane / 4
+// and lane / 4 + 8: per store instruction the eight rows of a warp fall in distinct 16-byte pieces of distinct bank
+// halves, no bank conflict (tests/test_fp8_static_host.py models the layout).  Columns N .. 64 ceil(N / 64) - 1 are
+// written as 0 (the consumer reads whole 64-byte chunks, and a stale byte could be an e4m3 NaN), including the second
+// half of the group at block_n 32 (the host allows that width for N <= 32 only).
+__device__ __forceinline__ uint32_t e4m3x2_rn(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+template <int S>
+__device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
+                                                       const TileCoord& c, int warp, int lane) {
+  constexpr int BN = 2 * S;
+  const int n_pad = (d.n_logical + 63) & ~63;
+  const int r0 = lane >> 2, q = lane & 3;
+  const uint32_t swz = (r0 >> 1) & 3;          // rows r0 and r0 + 8 share it
+  const float rn = d.out_ratio;
+  for (int g = 0; 64 * g < (BN < 64 ? 64 : BN); ++g) {
+    const int lcol = c.n0 + g * 64;
+    if (lcol >= n_pad) break;
+    const int tile = epi_stage_acquire(e, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v[16];
+      if (64 * g + 32 * h < BN) {
+        acc_chunk(2 * g + h, acc, v);
+        epi_dequant(d, v, lcol + 32 * h + 2 * q, d.a_scale);
+        epi_frag(d, v, lcol + 32 * h + 2 * q, false);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int col = lcol + 32 * h + 8 * j + 2 * q;
+        uint32_t lo = 0, hi = 0;
+        if (64 * g + 32 * h < BN) {
+          lo = e4m3x2_rn(col < d.n_logical ? __fmul_rn(v[4 * j], rn) : 0.f,
+                         col + 1 < d.n_logical ? __fmul_rn(v[4 * j + 1], rn) : 0.f);
+          hi = e4m3x2_rn(col < d.n_logical ? __fmul_rn(v[4 * j + 2], rn) : 0.f,
+                         col + 1 < d.n_logical ? __fmul_rn(v[4 * j + 3], rn) : 0.f);
+        }
+        const int b = 32 * h + 8 * j + 2 * q;  // byte within the 64-byte row segment
+        const uint32_t off = static_cast<uint32_t>((((b >> 4) ^ swz) << 4) | (b & 15));
+        uint8_t* t = e.stg_ptr + tile;
+        *reinterpret_cast<uint16_t*>(t + r0 * 64 + off) = static_cast<uint16_t>(lo);
+        *reinterpret_cast<uint16_t*>(t + (r0 + 8) * 64 + off) = static_cast<uint16_t>(hi);
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      epi_tma_store(d, e, e.stg_ptr + tile, c, warp, lcol);
       bulk_commit();
     }
   }
@@ -1141,7 +1203,10 @@ __device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&f
 // F8: the E4M3 instantiation (pf_conv3_halo_e4m3_kernel, d.a_e4m3).  The sources are 64-channel segments of one e4m3
 // map, each k16 step becomes a k32 step (two per tap, wgmma.m64nBNk32.f32.e4m3.e4m3 with A from registers) and the
 // plain-output epilogue multiplies the accumulator by s_a[image] * s_w[column] before the bias.
-template <int CL, int BN, bool F8>
+//
+// Q8 (F8 only): the static-scale instantiation (pf_conv3_halo_e4m3_q8_kernel, d.a_static): one input scale d.a_scale
+// for the launch, and either the bf16 output or (d.out_e4m3) the e4m3 operand map of the next conv.
+template <int CL, int BN, bool F8, bool Q8 = false>
 __device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
   constexpr bool MC = CL > 1;
   constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1);
@@ -1322,7 +1387,10 @@ __device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
       // plain bf16 outputs (the host sets tma_out for the whole launch): fragment layout, stmatrix staging, bulk
       // stores of {G ch, 8 px, 2 rows} boxes (TMA clips pixels past W / H, columns past the output and the phantom
       // img >= NB tile of a cluster); everything else row per thread
-      if constexpr (F8) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, true>(d, et, acc, c, warp, lane);
+      if constexpr (Q8) {
+        if (d.out_e4m3) epilogue_tile_tma_e4m3(d, et, acc, c, warp, lane);
+        else epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, 2>(d, et, acc, c, warp, lane);
+      } else if constexpr (F8) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, 1>(d, et, acc, c, warp, lane);
       else if (d.tma_out) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64>(d, et, acc, c, warp, lane);
       else epilogue_tile(d, c, acc, warp, lane, buf, nullptr);
       __syncwarp();
@@ -1344,6 +1412,10 @@ template <int CL, int BN>
 __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_kernel(const __grid_constant__ GemmKernelParams P) {
   conv3_halo_body<CL, BN, true>(P);
 }
+template <int CL, int BN>
+__global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_q8_kernel(const __grid_constant__ GemmKernelParams P) {
+  conv3_halo_body<CL, BN, true, true>(P);
+}
 
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1363,11 +1435,25 @@ static KernelFn halo_kernel_cl(int bn) {
     default: return nullptr;
   }
 }
+template <int CL>
+static KernelFn halo_q8_kernel_cl(int bn) {
+  switch (bn) {
+    case 32: return pf_conv3_halo_e4m3_q8_kernel<CL, 32>;
+    case 64: return pf_conv3_halo_e4m3_q8_kernel<CL, 64>;
+    case 128: return pf_conv3_halo_e4m3_q8_kernel<CL, 128>;
+    case 192: return pf_conv3_halo_e4m3_q8_kernel<CL, 192>;
+    default: return nullptr;
+  }
+}
 template <bool F8>
 static KernelFn halo_kernel_t(int cl, int bn) {
   return cl == 4 ? halo_kernel_cl<4, F8>(bn) : (cl == 2 ? halo_kernel_cl<2, F8>(bn) : halo_kernel_cl<1, F8>(bn));
 }
-static KernelFn halo_kernel(int cl, int bn, bool f8 = false) { return f8 ? halo_kernel_t<true>(cl, bn) : halo_kernel_t<false>(cl, bn); }
+// q8: pf_conv3_halo_e4m3_q8_kernel (static input scale), f8 must be set too
+static KernelFn halo_kernel(int cl, int bn, bool f8 = false, bool q8 = false) {
+  if (q8) return cl == 4 ? halo_q8_kernel_cl<4>(bn) : (cl == 2 ? halo_q8_kernel_cl<2>(bn) : halo_q8_kernel_cl<1>(bn));
+  return f8 ? halo_kernel_t<true>(cl, bn) : halo_kernel_t<false>(cl, bn);
+}
 // pf_gemm_kernel<MC, bn> for the widths of kGemmWidths, nullptr otherwise
 template <bool MC>
 static KernelFn gemm_kernel_mc(int bn) {
@@ -1395,10 +1481,11 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
         if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_kernel(mc, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (bool mc : {false, true})
       if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_pp_kernel(mc), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
-    for (bool f8 : {false, true})
+    for (int v = 0; v < 3; ++v)
       for (int cl : {1, 2, 4})
         for (int bn : {32, 64, 128, 192})
-          if (e == cudaSuccess) e = cudaFuncSetAttribute(halo_kernel(cl, bn, f8), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+          if (e == cudaSuccess)
+            e = cudaFuncSetAttribute(halo_kernel(cl, bn, v > 0, v > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm kernels): %s", cudaGetErrorString(e));
     cudaDeviceGetAttribute(&g_sm_counts[dev], cudaDevAttrMultiProcessorCount, dev);
     attr_done[dev] = true;
@@ -1409,7 +1496,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     int ktrue = 0;
     for (int s = 0; s < d.num_src; ++s) ktrue += d.k_true[s];
     const int n_true = d.ps > 1 ? d.n_logical * d.ps * d.ps : d.N;
-    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? "conv3x3_e4m3" : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : "linear")),
+    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? (d.a_static ? (d.out_e4m3 ? "conv3x3_e4m3_static_q8out" : "conv3x3_e4m3_static") : "conv3x3_e4m3") : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : "linear")),
               rows, d.taps, ktrue, n_true, d.act ? (d.act == PF_ACT_GELU ? " gelu" : (d.act == PF_ACT_RELU ? " relu" : " softplus")) : "",
               d.gamma ? " gamma" : (d.vt ? " vt" : ""), d.w2 ? " tail" : "");
   }
@@ -1428,8 +1515,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   if (P.total_tiles <= 0 || ks <= 0) return set_error("gemm: empty problem");
   int grid = P.total_tiles < g_sm_count ? P.total_tiles : g_sm_count;
   if (d.halo) {
-    const bool f8 = d.a_e4m3 != 0;
-    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n, f8);
+    const bool f8 = d.a_e4m3 != 0, q8 = f8 && d.a_static != 0;
+    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n, f8, q8);
     if (hk == nullptr) return set_error("conv3 halo: block_n %d (32, 64, 128 or 192)", d.block_n);
     const int b_bytes = halo_kc(d.block_n, f8) * d.block_n * kBlockK * (f8 ? 1 : 2);     // one weight stage
     const int hstages = halo_stages(d.block_n, f8);
@@ -1450,8 +1537,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       at[1].val.programmaticStreamSerializationAllowed = 1;
       cfg.attrs = at;
       cfg.numAttrs = 1;
-      static int max_clusters[kMaxDevices][2][5] = {};
-      int (&mcl)[5] = max_clusters[dev][f8 ? 1 : 0];
+      static int max_clusters[kMaxDevices][3][5] = {};
+      int (&mcl)[5] = max_clusters[dev][q8 ? 2 : (f8 ? 1 : 0)];
       if (mcl[cl] == 0) {
         cfg.gridDim = dim3(cl * (g_sm_count / cl));
         int n = 0;
@@ -1466,7 +1553,9 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     } else {
       le = launch_pdl(hk, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
     }
-    if (le != cudaSuccess) return set_error("%s launch: %s", f8 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel", cudaGetErrorString(le));
+    if (le != cudaSuccess)
+      return set_error("%s launch: %s", q8 ? "pf_conv3_halo_e4m3_q8_kernel" : (f8 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel"),
+                       cudaGetErrorString(le));
   } else {
     if (d.pp && (d.block_n % kPpBN != 0 || d.num_src != 1 || d.a_mode != 0 || !d.tma_out))
       return set_error("gemm: the ping-pong kernel takes plain linear layers at block_n 128 / 256 (block_n %d)", d.block_n);
@@ -1497,7 +1586,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(e));
-  count_launch(d.halo ? (d.a_e4m3 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel")
+  count_launch(d.halo ? (d.a_e4m3 ? (d.a_static ? "pf_conv3_halo_e4m3_q8_kernel" : "pf_conv3_halo_e4m3_kernel") : "pf_conv3_halo_kernel")
                        : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"));
   return 0;
 }

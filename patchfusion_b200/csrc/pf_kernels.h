@@ -51,6 +51,13 @@ struct GemmDesc {
   int a_e4m3;
   const float* s_a;
   const float* s_w;
+  // static input scale (pf_conv3_halo_e4m3_q8_kernel): a_scale for every tile instead of s_a[img]; out_e4m3: the output
+  // is an e4m3 map written as e4m3_rn(sat(v * out_ratio)) through a uint8 tensor map, pad columns up to 64 ceil(N / 64)
+  // zero
+  int a_static;
+  float a_scale;
+  int out_e4m3;
+  float out_ratio;
 };
 
 int set_error(const char* fmt, ...);

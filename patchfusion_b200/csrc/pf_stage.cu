@@ -31,6 +31,7 @@ struct Ctx {
   int err;
   pf_tap_fn tap; void* tap_user;
   int n_e4m3;           // FP8 convs issued so far (names their debug taps)
+  const char* lname;    // name of the U-Net conv being issued (FP8_LAYERS in params.py), for the calibration taps
 
   void* alloc(size_t bytes) {
     off = (off + 255) & ~static_cast<size_t>(255);
@@ -127,6 +128,12 @@ static void conv_into_e4m3(Ctx& c, const pf_layer& L, const Map* const* srcs, in
   for (int i = 0; i < ns; ++i) { p[i] = srcs[i]->p; cc[i] = srcs[i]->C; ld[i] = srcs[i]->ld; }
   if (c.live()) c.chk(pf_quantize_e4m3_tiles(ns, p, cc, ld, T, H, W, part, q, s_a, c.stream));
   if (!c.live()) return;
+  // calibration tap "amax.<layer>": the tiles' partial maxima [T, PF_QUANT_PARTS] of the input this conv quantized
+  if (c.tap != nullptr && c.lname != nullptr) {
+    char an[32];
+    snprintf(an, sizeof(an), "amax.%s", c.lname);
+    c.tap_out(an, part, 1, T, PF_QUANT_PARTS, PF_QUANT_PARTS);
+  }
   pf_gemm_desc d;
   memset(&d, 0, sizeof(d));
   d.num_src = ns; d.a_mode = 1;
@@ -151,9 +158,72 @@ static void conv_into_e4m3(Ctx& c, const pf_layer& L, const Map* const* srcs, in
   ++c.n_e4m3;
 }
 
+// ---- fusion_precision 'fp8_static': one calibrated amax per conv input (pf_layer.a_amax), fixed before the forward.
+// r = 448 / amax and scale = amax / 448, one IEEE fp32 division each, as the kernels' per-tile rule.
+static float static_ratio(float amax) { return amax == 0.f ? 0.f : 448.f / amax; }
+static float static_scale(float amax) { return amax / 448.f; }
+
+// the sources quantized at L's static ratio into one e4m3 map of kc bytes per pixel (one launch)
+static void* quant_static(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, int* kc) {
+  const int T = srcs[0]->B, H = srcs[0]->H, W = srcs[0]->W;
+  *kc = 0;
+  for (int i = 0; i < ns; ++i) *kc += pad_to(srcs[i]->C, 64);
+  void* q = c.alloc(static_cast<size_t>(T) * H * W * *kc);
+  if (!c.live()) return q;
+  const void* p[3] = {nullptr, nullptr, nullptr};
+  int32_t cc[3] = {0, 0, 0}, ld[3] = {0, 0, 0};
+  for (int i = 0; i < ns; ++i) { p[i] = srcs[i]->p; cc[i] = srcs[i]->C; ld[i] = srcs[i]->ld; }
+  c.chk(pf_quantize_e4m3_static(ns, p, cc, ld, T, H, W, static_ratio(*L.a_amax), q, c.stream));
+  return q;
+}
+
+// the static-scale E4M3 conv (pf_conv3_halo_e4m3_q8_kernel) over the e4m3 map q (sources of src_c channels, kc bytes
+// per pixel) with ReLU: a bf16 output, or, when `next` is given, next's e4m3 operand map (out_ld = its kc bytes) at
+// next's static ratio.  Debug taps "e4m3s.<layer>.in.<H>x<W>" (the e4m3 map the conv read) and
+// "e4m3s.<layer>.out.<H>x<W>" (what it wrote), so a test can check each conv on exactly its input.
+static void conv_static_e4m3(Ctx& c, const pf_layer& L, const void* q, int kc, const int* src_c, int ns, int T, int H,
+                             int W, void* out, int out_ld, const pf_layer* next) {
+  if (!c.live()) return;
+  pf_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.num_src = ns; d.a_mode = 1;
+  d.a_ptr[0] = q;
+  for (int i = 0; i < ns; ++i) { d.a_c[i] = pad_to(src_c[i], 8); d.a_ld[i] = kc; }
+  d.NB = T; d.H = H; d.W = W;
+  GemmOpt o; o.act = PF_ACT_RELU;
+  gemm_desc_common(d, L, o, out, 0, out_ld);
+  d.w_ptr = L.w8;
+  d.a_e4m3 = 1; d.s_w = L.w_scale;
+  d.a_static = 1; d.a_scale = static_scale(*L.a_amax);
+  if (next != nullptr) { d.out_e4m3 = 1; d.out_ratio = static_ratio(*next->a_amax); }
+  c.chk(pf_gemm(&d, c.stream));
+  if (c.tap != nullptr && c.live() && c.lname != nullptr) {
+    char nm[48];
+    const long long rows = static_cast<long long>(T) * H * W;
+    snprintf(nm, sizeof(nm), "e4m3s.%s.in.%dx%d", c.lname, H, W);
+    c.tap_out(nm, q, 2, rows, kc, kc);
+    snprintf(nm, sizeof(nm), "e4m3s.%s.out.%dx%d", c.lname, H, W);
+    if (next != nullptr) c.tap_out(nm, out, 2, rows, out_ld, out_ld);
+    else c.tap_out(nm, out, 0, rows, L.N, out_ld);
+  }
+}
+
 // 3x3 / 1x1 conv over up to three channel-concatenated NHWC sources
 static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_f32, int out_ld,
                       const GemmOpt& o = GemmOpt()) {
+  if (L.w_scale != nullptr && L.a_amax != nullptr && L.taps == 9 && !out_f32) {
+    // a static conv whose producer wrote bf16 (the second conv after a fused-resample first one): one quantize pass
+    if (o.act != PF_ACT_RELU || o.res1 || o.res2 || o.relu_copy || o.tail || o.gamma) {
+      c.chk(set_error("static FP8 conv: plain ReLU output only"));
+      return;
+    }
+    int kc = 0;
+    void* q = quant_static(c, L, srcs, ns, &kc);
+    int cs[3] = {0, 0, 0};
+    for (int i = 0; i < ns; ++i) cs[i] = srcs[i]->C;
+    conv_static_e4m3(c, L, q, kc, cs, ns, srcs[0]->B, srcs[0]->H, srcs[0]->W, out, out_ld, nullptr);
+    return;
+  }
   if (L.w_scale != nullptr && L.taps == 9 && !out_f32) {
     conv_into_e4m3(c, L, srcs, ns, out, out_ld, o);
     return;
@@ -173,7 +243,7 @@ static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns,
 // materialised; sources already at (H, W) are read directly.  Opt-in (PF_OPT_FUSED_RESAMPLE = 1): two producer warps per
 // CTA cannot keep up with the tensor pipe (measured 215 -> 317 ms per 4K image), so the default materialises them.
 static Map resize(Ctx& c, const Map& x, int OH, int OW);
-static Map conv_resampled(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, int H, int W, const GemmOpt& o = GemmOpt()) {
+static Map conv_resampled(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, int H, int W, const GemmOpt& o) {
   Map out = c.map(srcs[0]->B, H, W, L.N);
   if (L.taps != 9 || !option(PF_OPT_FUSED_RESAMPLE)) {
     Map tmp[3];
@@ -209,6 +279,52 @@ static Map conv(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, const
 static Map conv1(Ctx& c, const pf_layer& L, const Map& s, const GemmOpt& o = GemmOpt()) {
   const Map* a[1] = {&s};
   return conv(c, L, a, 1, o);
+}
+
+// One DoubleConv of the U-Net, X.0 -> ReLU -> X.1 -> ReLU (guided_fusion_model.py DoubleConv), over sources read at
+// (H, W) (resampled: through F.interpolate(bilinear, align_corners=True) when their size differs).  `name` is the
+// DoubleConv's name in FP8_LAYERS (inc, down<i>, up<i>, cv<i>).  When both convs have static scales ('fp8_static') X.0
+// reads its sources through one pf_quantize_e4m3_static and writes X.1's e4m3 operand directly: X.0's output has no
+// other consumer, so no bf16 map of it exists.  Otherwise (and for a fused-resample X.0, which stays bf16) the two convs
+// run one after the other as before.
+static Map resize(Ctx& c, const Map& x, int OH, int OW);
+static Map conv_resampled(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, int H, int W, const GemmOpt& o);
+static Map double_conv(Ctx& c, const pf_layer& L0, const pf_layer& L1, const Map* const* srcs, int ns, int H, int W,
+                       bool resampled, const char* name) {
+  GemmOpt gr; gr.act = PF_ACT_RELU;
+  char n0[24], n1[24];
+  snprintf(n0, sizeof(n0), "%s.0", name);
+  snprintf(n1, sizeof(n1), "%s.1", name);
+  const bool st = L0.w_scale && L1.w_scale && L0.a_amax && L1.a_amax && L0.taps == 9 && L1.taps == 9;
+  if (!st || (resampled && option(PF_OPT_FUSED_RESAMPLE))) {
+    c.lname = n0;
+    Map y = resampled ? conv_resampled(c, L0, srcs, ns, H, W, gr) : conv(c, L0, srcs, ns, gr);
+    c.lname = n1;
+    Map x = conv1(c, L1, y, gr);
+    c.lname = nullptr;
+    return x;
+  }
+  Map tmp[3];
+  const Map* a[3];
+  int cs[3] = {0, 0, 0};
+  for (int i = 0; i < ns; ++i) {
+    tmp[i] = resampled ? resize(c, *srcs[i], H, W) : *srcs[i];
+    a[i] = &tmp[i];
+    cs[i] = srcs[i]->C;
+  }
+  const int T = srcs[0]->B;
+  int kc0 = 0;
+  void* q0 = quant_static(c, L0, a, ns, &kc0);
+  const int kc1 = pad_to(L0.N, 64);
+  void* q1 = c.alloc(static_cast<size_t>(T) * H * W * kc1);
+  Map out = c.map(T, H, W, L1.N);
+  c.lname = n0;
+  conv_static_e4m3(c, L0, q0, kc0, cs, ns, T, H, W, q1, kc1, &L1);
+  c.lname = n1;
+  const int c1[1] = {L0.N};
+  conv_static_e4m3(c, L1, q1, kc1, c1, 1, T, H, W, out.p, out.ld, nullptr);
+  c.lname = nullptr;
+  return out;
 }
 
 // F.interpolate(mode='bilinear', align_corners=True)
@@ -509,16 +625,17 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
   Map u = c.map(T, H, W, 5);
   if (c.live()) c.chk(pf_pack_unet_input(droi, fine_depth, crops, T, H, W, u.p, u.ld, c.stream));
   // encoder (guided_fusion_model.py:179-184)
-  GemmOpt gr; gr.act = PF_ACT_RELU;
-  Map x = conv1(c, Wf.inc[0], u, gr);
-  x = conv1(c, Wf.inc[1], x, gr);
+  const Map* ui[1] = {&u};
+  Map x = double_conv(c, Wf.inc[0], Wf.inc[1], ui, 1, H, W, false, "inc");
   Map enc[6];
   enc[5] = x;
   for (int i = 0; i < 5; ++i) {
     Map p = c.map(T, x.H / 2, x.W / 2, x.C);
     if (c.live()) c.chk(pf_maxpool2(x.p, T, x.H, x.W, pad_to(x.C, 8), x.ld, p.p, p.ld, c.stream));
-    x = conv1(c, Wf.down[i][0], p, gr);
-    x = conv1(c, Wf.down[i][1], x, gr);
+    const Map* pi[1] = {&p};
+    char nm[8];
+    snprintf(nm, sizeof(nm), "down%d", i);
+    x = double_conv(c, Wf.down[i][0], Wf.down[i][1], pi, 1, p.H, p.W, false, nm);
     enc[4 - i] = x;
   }
   // decoder, low -> high resolution (guided_fusion_model.py:188-205)
@@ -529,20 +646,20 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
     // F.interpolate(enc / previous level / guide, size=(h, w), bilinear, align_corners=True) feeding the 3x3 convs
     // (guided_fusion_model.py:98-99,191-203)
     Map e = enc[i];
+    char nm[8];
     if (i > 0) {
       const Map* a[3] = {&enc[i], &prev, &guide[i - 1]};
-      e = conv_resampled(c, Wf.up[i - 1][0], a, 3, h, w, gr);
-      e = conv1(c, Wf.up[i - 1][1], e, gr);
+      snprintf(nm, sizeof(nm), "up%d", i);
+      e = double_conv(c, Wf.up[i - 1][0], Wf.up[i - 1][1], a, 3, h, w, true, nm);
     }
     Map cr = c.map(T, h, w, gm.C);
     if (c.live())
       c.chk(pf_roi_crop_zoom_batched(gm.p, 0, h, w, pad_to(gm.C, 8), gm.ld, tile_image, boxes, T, static_cast<float>(h) / H,
                                      cr.p, cr.ld, 0, c.stream));
     const Map* a2[2] = {&e, &cr};
-    Map y = conv_resampled(c, Wf.cv[i][0], a2, 2, h, w, gr);
-    prev = conv1(c, Wf.cv[i][1], y, gr);
+    snprintf(nm, sizeof(nm), "cv%d", i);
+    prev = double_conv(c, Wf.cv[i][0], Wf.cv[i][1], a2, 2, h, w, true, nm);
     outs[i] = prev;
-    char nm[16];
     snprintf(nm, sizeof(nm), "fuse%d", i);
     c.tap_out(nm, prev.p, 0, prev.rows(), prev.C, prev.ld);
   }
@@ -552,7 +669,7 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
 static Ctx make_ctx(void* ws, size_t bytes, bool dry, void* stream, pf_tap_fn tap, void* user) {
   Ctx c;
   c.base = static_cast<uint8_t*>(ws); c.cap = bytes; c.off = 0; c.dry = dry; c.stream = stream; c.err = 0;
-  c.tap = tap; c.tap_user = user; c.n_e4m3 = 0;
+  c.tap = tap; c.tap_user = user; c.n_e4m3 = 0; c.lname = nullptr;
   return c;
 }
 

@@ -23,7 +23,8 @@ import torch.nn.functional as F
 
 from . import lib, ops
 from .ops import ACT_GELU, ACT_NONE, ACT_RELU, ACT_SOFTPLUS, call, pad_to, stream_ptr
-from .params import WINDOW, branch_hparams, fusion_precision, guided_fusion_hparams, normed_attractors, _get
+from .params import FP8_LAYERS, WINDOW, branch_hparams, fusion_fp8_amax, fusion_precision, guided_fusion_hparams, \
+    normed_attractors, _get
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -72,6 +73,15 @@ class Engine:
         self.sd = None   # fp32 originals are no longer needed on the device
         self.c_branch = {b: self._c_branch(b) for b in ('coarse', 'fine') if b in self.parts}
         self.c_fusion = self._c_fusion() if 'fusion' in self.parts else None
+        # 'fp8_static': c_fusion carries the calibrated input amax of each FP8 conv (set_fp8_amax); c_fusion_tiles is the
+        # same stage with per-tile scales, which calibration runs.  `calib` (a dict while PatchFusion.calibrate_fp8 runs)
+        # collects each conv's input amax from the per-tile stage.
+        self.c_fusion_tiles = self.c_fusion
+        self.fp8_static = 'fusion' in self.parts and fusion_precision(config) == 'fp8_static'
+        self.fp8_amax = None
+        self.calib = None
+        if self.fp8_static:
+            self.set_fp8_amax(fusion_fp8_amax(config))
 
     # ------------------------------------------------------------------ buffers
     def buf(self, key, shape, dtype=BF16):
@@ -193,10 +203,10 @@ class Engine:
         hp = self.hp['fine']
         C = hp['features']
         Wd = {}
-        # fusion_precision 'fp8': the U-Net's 3x3 convs get e4m3 panels; the convs whose input can come through the
+        # fusion_precision 'fp8' / 'fp8_static': the U-Net's 3x3 convs get e4m3 panels; the convs whose input can come through the
         # fused resample (up*.0, cv*.0) keep their bf16 panel for that path too.  fusion_conv_list, G2L and the head
         # stay bf16.
-        f8 = 'only' if fusion_precision(self.cfg) == 'fp8' else None
+        f8 = 'only' if fusion_precision(self.cfg) in ('fp8', 'fp8_static') else None
         f8rs = 'keep_bf16' if f8 else None
         for i in range(5):      # level 5's fused map is dead in the U-Net (guided_fusion_model.py:198)
             Wd['fc%d' % i] = self._conv('fusion_conv_list.%d' % i, src_c=[C, C])
@@ -304,7 +314,29 @@ class Engine:
         B.head = self._c_head(Wd['head'], hp, self.bcfg[which], True, self.bcfg[which])
         return B
 
-    def _c_fusion(self):
+    def set_fp8_amax(self, table):
+        """'fp8_static': the calibrated input amax of the 34 FP8 convs ({name: float}, validated) that the stage runs
+        with, or None (no table: the fusion stage refuses to run, calibration still can).  The values are read when a
+        stage is issued, so graphs captured before a change must be dropped (PatchFusion.engine does)."""
+        if table is None:
+            self.fp8_amax, self.c_fusion = None, self.c_fusion_tiles
+            return
+        table = dict(table)
+        arr = (ct.c_float * len(FP8_LAYERS))(*[table[k] for k in FP8_LAYERS])
+        self._keep.append(arr)
+        self.c_fusion = self._c_fusion({k: ct.addressof(arr) + 4 * i for i, k in enumerate(FP8_LAYERS)})
+        self.fp8_amax = table
+
+    def _fusion_struct(self):
+        if self.calib is not None:
+            return self.c_fusion_tiles
+        if self.fp8_static and self.fp8_amax is None:
+            raise RuntimeError("fusion_precision 'fp8_static' needs the calibrated input scales `fusion_fp8_amax`: run "
+                               "PatchFusion.calibrate_fp8 (or tools/calibrate_fp8.py) first")
+        return self.c_fusion
+
+    def _c_fusion(self, amax=None):
+        """amax: {FP8 layer name: address of its fp32 amax} of a calibrated 'fp8_static' stage, or None"""
         from . import stage
         Wf = self.W['fusion']
         F_ = stage.PfFusion()
@@ -329,6 +361,13 @@ class Engine:
             self._keep.append(blocks)
             g.blocks = blocks
         F_.head = self._c_head(Wf['head'], self.hp['coarse'], self.bcfg['coarse'], False, self.cfg)
+        if amax is not None:
+            for i in range(5):
+                F_.down[i][0].a_amax, F_.down[i][1].a_amax = amax['down%d.0' % i], amax['down%d.1' % i]
+                F_.up[i][0].a_amax, F_.up[i][1].a_amax = amax['up%d.0' % (i + 1)], amax['up%d.1' % (i + 1)]
+            F_.inc[0].a_amax, F_.inc[1].a_amax = amax['inc.0'], amax['inc.1']
+            for i in range(6):
+                F_.cv[i][0].a_amax, F_.cv[i][1].a_amax = amax['cv%d.0' % i], amax['cv%d.1' % i]
         return F_
 
     # ------------------------------------------------------------------ workspaces (one arena per stage role)
@@ -356,8 +395,21 @@ class Engine:
 
     def _tap_cb(self, arena, taps):
         def cb(user, name, ptr, is_f32, rows, cols, ld):
-            t = self._view(arena, ptr, (rows, ld), F32 if is_f32 else BF16)
+            # is_f32: 0 bf16, 1 fp32, 2 e4m3 bytes (the static FP8 convs' operand maps)
+            t = self._view(arena, ptr, (rows, ld), (BF16, F32, torch.uint8)[is_f32])
             taps[name.decode()] = t[:, :cols].clone()
+        return cb
+
+    def _calib_cb(self, arena):
+        """calibration: fold each FP8 conv's per-tile partial maxima (tap "amax.<layer>") into calib[layer], on the
+        device and NaN-propagating"""
+        def cb(user, name, ptr, is_f32, rows, cols, ld):
+            name = name.decode()
+            if not name.startswith('amax.'):
+                return
+            m = self._view(arena, ptr, (rows, ld), F32)[:, :cols].amax()
+            k = name[5:]
+            self.calib[k] = m if k not in self.calib else torch.maximum(self.calib[k], m)
         return cb
 
     # ------------------------------------------------------------------ stages (sequenced inside libpf_b200)
@@ -415,7 +467,7 @@ class Engine:
 
     def fusion_bytes(self, T, g2l_maps):
         from . import stage
-        return stage.fusion_workspace_bytes(self.c_fusion, T, self._pf_maps(g2l_maps))
+        return stage.fusion_workspace_bytes(self._fusion_struct(), T, self._pf_maps(g2l_maps))
 
     def fusion(self, crops, boxes, fine_depth, fine_feats, coarse_depth, coarse_feats, g2l_maps, taps=None,
                depth_out=None, ws=None, tile_image=None):
@@ -426,7 +478,8 @@ class Engine:
         T = crops.shape[0]
         H, W = self.P
         gm = self._pf_maps(g2l_maps)
-        need = stage.fusion_workspace_bytes(self.c_fusion, T, gm)
+        cfu = self._fusion_struct()
+        need = stage.fusion_workspace_bytes(cfu, T, gm)
         if ws is None:
             arena, off = self.arena('fusion', need), 0
         else:
@@ -440,7 +493,9 @@ class Engine:
         if tile_image is not None:
             assert tile_image.dtype == torch.int32 and tile_image.is_contiguous() and tile_image.numel() == T
         tap = self._tap_cb(arena, taps) if taps is not None else None
-        stage.fusion_forward(self.c_fusion, crops, boxes, T, fine_depth, self._pf_maps(fine_feats), coarse_depth,
+        if tap is None and self.calib is not None:
+            tap = self._calib_cb(arena)
+        stage.fusion_forward(cfu, crops, boxes, T, fine_depth, self._pf_maps(fine_feats), coarse_depth,
                              self._pf_maps(coarse_feats), gm, arena.data_ptr() + off, need, depth_out, tap,
                              tile_image=tile_image)
         if taps is not None:

@@ -44,6 +44,7 @@ class GemmDesc(C.Structure):
         ('out3', C.c_void_p), ('out3_ld', C.c_int32),
         ('rs_h', C.c_int32 * 3), ('rs_w', C.c_int32 * 3),
         ('a_e4m3', C.c_int32), ('s_a', C.c_void_p), ('s_w', C.c_void_p),
+        ('a_static', C.c_int32), ('a_scale', C.c_float), ('out_e4m3', C.c_int32), ('out_ratio', C.c_float),
     ]
 
 
@@ -66,6 +67,8 @@ SIGNATURES = {
     'pf_pack_weight_e4m3': [_p, _i, _i, _i, C.POINTER(C.c_int32), _i, _p, _p, _p, _p],
     'pf_quantize_e4m3_tiles': [_i, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _i, _i, _p,
                                _p, _p, _p],
+    'pf_quantize_e4m3_static': [_i, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _i, _i, _f,
+                                _p, _p],
     'pf_layernorm': [_p, _i, _p, _p, _f, _i, _i, _p, _i, _p],
     'pf_layernorm_grouped': [_p, _i, _p, _p, _f, _i, _i, _i, _i, _i, _p, _i, _p],
     'pf_attention': [_p, _i, _p, _i, _i, _i, _i, _f, _p, _i, _p],

@@ -13,7 +13,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .params import ParamTree, _get, fusion_precision, state_layout, synthetic_state_dict, relative_position_index
+from .params import FP8_LAYERS, ParamTree, _get, fusion_fp8_amax, fusion_precision, state_layout, synthetic_state_dict, relative_position_index
 
 try:
     from huggingface_hub import PyTorchModelHubMixin
@@ -506,7 +506,8 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         self.patch_process_shape = config.patch_process_shape
         self.tile_cfg = self.prepare_tile_cfg(config.image_raw_shape, config.patch_split_num)
         self.coarse_branch_cfg = config.coarse_branch
-        self.fusion_precision = fusion_precision(config)     # ValueError on anything but 'bf16' / 'fp8'
+        self.fusion_precision = fusion_precision(config)     # ValueError on anything but 'bf16' / 'fp8' / 'fp8_static'
+        fusion_fp8_amax(config)                              # ValueError on a malformed calibration table
         for br in (config.coarse_branch, config.fine_branch):
             if br.type not in ('ZoeDepth', 'DA-ZoeDepth'):
                 raise NotImplementedError
@@ -556,7 +557,49 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
                 raise RuntimeError('PatchFusion (H100): the hot path runs on libpf_b200 only; move the model to a '
                                    'CUDA device (there is no CPU fallback)')
             self._engine = Engine(self.config, self.state_dict(), p.device)
+        elif self._engine.fp8_static:
+            # the calibration table is part of the config: a changed table re-points the stage and drops the graphs
+            # captured with the old scales
+            table = fusion_fp8_amax(self.config)
+            if table != self._engine.fp8_amax:
+                self._engine.set_fp8_amax(table)
+                self._graphs = {}
         return self._engine
+
+    @torch.no_grad()
+    def calibrate_fp8(self, image_lr, image_hr, cai_mode='m1', process_num=4, tile_cfg=None, reset=False):
+        """Post-training calibration of the static FP8 U-Net ('fp8' and 'fp8_static' models): runs forward(mode='infer')
+        on the given images (the same arguments: batches, mixed geometry, rN modes drawing from `random`) with the
+        per-tile 'fp8' arithmetic on this model's panels, and takes, for each of the 34 FP8 convs, the maximum over all
+        tiles of its input's amax.  That is merged by max into config['fusion_fp8_amax'] (reset=True starts from an
+        empty table), which 'fp8_static' then runs with, and returned.  Runs eagerly: no graph of it is kept, and the
+        graphs of earlier forwards are dropped."""
+        if self.fusion_precision not in ('fp8', 'fp8_static'):
+            raise ValueError("calibrate_fp8 needs fusion_precision 'fp8' or 'fp8_static' (this model: %r)"
+                             % self.fusion_precision)
+        eng = self.engine()
+        eng.calib = {}
+        graphs, self.use_cuda_graphs = self.use_cuda_graphs, False
+        try:
+            self.forward('infer', image_lr, image_hr, tile_cfg=tile_cfg, cai_mode=cai_mode, process_num=process_num)
+            found = {k: v.item() for k, v in eng.calib.items()}
+        finally:
+            eng.calib = None
+            self.use_cuda_graphs = graphs
+            self._graphs = {}
+        missing = [k for k in FP8_LAYERS if k not in found]
+        if missing:
+            raise RuntimeError('calibrate_fp8: no input amax for %s (a conv read through PF_OPT_FUSED_RESAMPLE has no '
+                               'materialised input to measure)' % missing)
+        table = {} if reset else dict(fusion_fp8_amax(self.config) or {})
+        for k in FP8_LAYERS:
+            table[k] = max(table.get(k, 0.0), found[k]) if found[k] == found[k] else found[k]
+        self.config['fusion_fp8_amax'] = fusion_fp8_amax(dict(fusion_fp8_amax=table))   # ValueError on NaN / inf
+        hub = getattr(self, '_hub_mixin_config', None)
+        if isinstance(hub, dict):                   # the config save_pretrained writes
+            hub['fusion_fp8_amax'] = dict(self.config['fusion_fp8_amax'])
+        self.engine()
+        return dict(self.config['fusion_fp8_amax'])
 
     def invalidate(self):
         super().invalidate()
@@ -859,6 +902,7 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         assert B >= 1 and image_lr.shape[0] == B, 'image_lr and image_hr must hold the same number (>= 1) of images'
         self._check_shard(shard, group)
         eng = self.engine()
+        eng._fusion_struct()            # 'fp8_static' without a calibration table: RuntimeError naming calibrate_fp8
         ph, pw = self.patch_process_shape
         plan_fn = None
         owner = shard is not None and self.shard_coarse == 'owner'

@@ -5,6 +5,7 @@ channel count tracked by the caller), token matrices `[rows, ld]`, fp32 where in
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import lib
@@ -126,6 +127,64 @@ def conv3_e4m3(pw, q, s_a, out, act=ACT_NONE, block_n=0):
     assert out.dtype == torch.bfloat16 and out.is_contiguous()
     d.out, d.out_ld = out.data_ptr(), out.shape[-1]
     d.a_e4m3, d.s_a, d.s_w = 1, s_a.data_ptr(), pw.w_scale.data_ptr()
+    call('pf_gemm', C.byref(d), stream_ptr())
+    return d
+
+
+def e4m3_static_ratio(amax):
+    """r = 448 / amax in fp32 (0 when amax == 0): the static quantize ratio of a calibrated amax (include/pf_b200.h)"""
+    a = np.float32(amax)
+    return float(np.float32(0.0) if a == 0 else np.float32(448.0) / a)
+
+
+def e4m3_static_scale(amax):
+    """amax / 448 in fp32: the dequantize scale of a calibrated amax"""
+    return float(np.float32(amax) / np.float32(448.0))
+
+
+def quantize_e4m3_static(srcs, amax, src_c=None, out=None):
+    """srcs: bf16 NHWC maps [T,H,W,ld_i] (logical channels src_c[i], default the last dim) -> the e4m3 map [T,H,W,Kc]
+    (uint8 storage, quantize_e4m3_tiles' layout) at the static ratio of `amax` (pf_quantize_e4m3_static, saturating)."""
+    T, H, W = srcs[0].shape[:3]
+    cs = [s_.shape[-1] for s_ in srcs] if src_c is None else list(src_c)
+    kc = sum(pad_to(c, 64) for c in cs)
+    for s_ in srcs:
+        assert s_.dtype == torch.bfloat16 and s_.is_contiguous() and tuple(s_.shape[:3]) == (T, H, W)
+    if out is None:
+        out = torch.empty((T, H, W, kc), dtype=torch.uint8, device=srcs[0].device)
+    assert out.dtype == torch.uint8 and tuple(out.shape) == (T, H, W, kc) and out.is_contiguous()
+    n = len(srcs)
+    ptrs = (C.c_void_p * 3)(*([s_.data_ptr() for s_ in srcs] + [None] * (3 - n)))
+    cc = (C.c_int32 * 3)(*(cs + [0] * (3 - n)))
+    ld = (C.c_int32 * 3)(*([s_.shape[-1] for s_ in srcs] + [0] * (3 - n)))
+    call('pf_quantize_e4m3_static', n, ptrs, cc, ld, T, H, W, e4m3_static_ratio(amax), out, stream_ptr())
+    return out
+
+
+def conv3_e4m3_static(pw, q, amax, out, next_amax=None, act=ACT_RELU, block_n=0):
+    """The static-scale E4M3 halo conv (pf_conv3_halo_e4m3_q8_kernel): q from quantize_e4m3_static at `amax`, pw from
+    pack_weight_e4m3.  next_amax None: out bf16 NHWC [T,H,W,ld]; else out is the uint8 e4m3 map [T,H,W,ld >= pad64(N)]
+    written at next_amax's ratio (the next conv's operand)."""
+    T, H, W, kc = q.shape
+    assert q.dtype == torch.uint8 and kc == sum(pad_to(c, 64) for c in pw.src_c) and pw.taps == 9
+    d = GemmDesc()
+    d.num_src = len(pw.src_c)
+    d.taps = 9
+    d.a_mode = 1
+    d.a_ptr[0] = q.data_ptr()
+    for i, c in enumerate(pw.src_c):
+        d.a_c[i], d.a_ld[i] = pad_to(c, 8), kc
+    d.NB, d.H, d.W = T, H, W
+    d.w_ptr = pw.w8.data_ptr()
+    d.N, d.Ktot, d.block_n = pw.N, pw.Ktot, block_n
+    d.bias = pw.bias.data_ptr() if pw.bias is not None else None
+    d.act = act
+    assert out.is_contiguous() and out.dtype == (torch.bfloat16 if next_amax is None else torch.uint8)
+    d.out, d.out_ld = out.data_ptr(), out.shape[-1]
+    d.a_e4m3, d.s_w = 1, pw.w_scale.data_ptr()
+    d.a_static, d.a_scale = 1, e4m3_static_scale(amax)
+    if next_amax is not None:
+        d.out_e4m3, d.out_ratio = 1, e4m3_static_ratio(next_amax)
     call('pf_gemm', C.byref(d), stream_ptr())
     return d
 

@@ -12,6 +12,7 @@ from the reference itself by oracle/make_golden.py.
 """
 from collections import OrderedDict
 import math
+import numbers
 
 import torch
 import torch.nn as nn
@@ -37,17 +38,44 @@ def _get(cfg, key, default=None):
     return getattr(cfg, key, default)
 
 
-FUSION_PRECISIONS = ('bf16', 'fp8')
+FUSION_PRECISIONS = ('bf16', 'fp8', 'fp8_static')
+# The Guided-Fusion U-Net's 34 3x3 convs that run E4M3 under 'fp8' / 'fp8_static', by their names in
+# Engine._pack_fusion: the two convs X.0 -> ReLU -> X.1 -> ReLU of each of the 17 DoubleConvs
+FP8_LAYERS = tuple(['inc.0', 'inc.1'] + ['down%d.%d' % (i, j) for i in range(5) for j in (0, 1)] +
+                   ['up%d.%d' % (i, j) for i in range(1, 6) for j in (0, 1)] +
+                   ['cv%d.%d' % (i, j) for i in range(6) for j in (0, 1)])
 
 
 def fusion_precision(config):
     """Top-level `fusion_precision`: what the Guided-Fusion U-Net's 3x3 convs (inc, down_conv_list, up_conv_list, convs)
     compute in.  'bf16' (default) is the path every other layer takes; 'fp8' runs them on E4M3 operands with one
-    scale per tile and input and one per output channel (include/pf_b200.h, DESIGN.md section 7)."""
+    scale per tile and input and one per output channel (include/pf_b200.h, DESIGN.md section 7); 'fp8_static' does
+    the same with one calibrated scale per conv input (`fusion_fp8_amax`, PatchFusion.calibrate_fp8)."""
     p = _get(config, 'fusion_precision', 'bf16')
     if p not in FUSION_PRECISIONS:
-        raise ValueError("fusion_precision should be one of 'bf16', 'fp8'")
+        raise ValueError("fusion_precision should be one of 'bf16', 'fp8', 'fp8_static'")
     return p
+
+
+def fusion_fp8_amax(config):
+    """Top-level `fusion_fp8_amax`: the calibrated amax of each FP8 conv's input, {layer name of FP8_LAYERS: float >= 0}
+    with exactly those 34 names, or None when the config has no table.  Anything else raises ValueError."""
+    t = _get(config, 'fusion_fp8_amax', None)
+    if t is None:
+        return None
+    if not isinstance(t, dict):
+        raise ValueError('fusion_fp8_amax should be a dict of the 34 FP8 layer names to their input amax')
+    missing = [k for k in FP8_LAYERS if k not in t]
+    unknown = sorted(str(k) for k in t if k not in FP8_LAYERS)
+    if missing or unknown:
+        raise ValueError('fusion_fp8_amax: missing layers %s, unknown layers %s' % (missing, unknown))
+    out = {}
+    for k in FP8_LAYERS:
+        v = t[k]
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
+            raise ValueError('fusion_fp8_amax[%r] = %r: a finite float >= 0 is required' % (k, v))
+        out[k] = float(v)
+    return out
 
 
 def branch_hparams(branch_cfg):

@@ -12,7 +12,8 @@ i32, f32, vp = C.c_int32, C.c_float, C.c_void_p
 
 class PfLayer(C.Structure):
     _fields_ = [('w', vp), ('bias', vp), ('N', i32), ('Ktot', i32), ('taps', i32), ('num_src', i32), ('src_c', i32 * 3),
-                ('ps', i32), ('ps_cout', i32), ('w2', vp), ('b2', vp), ('n2', i32), ('w8', vp), ('w_scale', vp)]
+                ('ps', i32), ('ps_cout', i32), ('w2', vp), ('b2', vp), ('n2', i32), ('w8', vp), ('w_scale', vp),
+                ('a_amax', vp)]
 
 
 class PfVitBlock(C.Structure):
