@@ -114,7 +114,11 @@ typedef struct pf_gemm_desc {
    * is ONE e4m3 NHWC map [NB, H, W, a_ld[0] bytes] holding the num_src sources back to back, each padded to 64 channels
    * (pf_quantize_e4m3_tiles); a_c[] still give the sources' channels.  w_ptr is an e4m3 panel (pf_pack_weight_e4m3).
    * The epilogue computes act(fl(acc * fl(s_a[img] * s_w[n])) + bias[n]): s_a one fp32 scale per image of the batch,
-   * s_w one per output channel. */
+   * s_w one per output channel.
+   * Linear layers (vit_precision 'fp8_static'; a_e4m3 and a_static set, a_mode 0, taps 1): a_ptr[0] is an e4m3 matrix
+   * [M, a_ld[0] bytes] of K = a_c[0] columns, K and N multiples of 128, one source, w_ptr the e4m3 panel [N_pad, K]; the
+   * outputs are the plain linear layer's (bf16, fp32, the gamma residual update, the V^T third of a fused qkv
+   * projection) or the e4m3 output below, after bias -> none / GELU / ReLU.  They run on pf_gemm_pp_e4m3_kernel. */
   int32_t a_e4m3;
   const float* s_a;
   const float* s_w;
@@ -123,7 +127,8 @@ typedef struct pf_gemm_desc {
    * bias[n]).  s_a may then be NULL.
    * E4M3 output (out_e4m3 != 0; needs a_static): the activated fp32 value v is written as q = e4m3_rn(sat(v * out_ratio))
    * (the consumer's r = 448 / amax, pf_quantize_e4m3_static's rule) into `out`, an e4m3 NHWC map [NB, H, W, out_ld
-   * bytes] whose columns N .. 64 ceil(N / 64) - 1 are written as zero: the operand map of a one-source E4M3 conv.
+   * bytes] whose columns N .. 64 ceil(N / 64) - 1 are written as zero: the operand map of a one-source E4M3 conv.  For
+   * a linear layer `out` is the e4m3 matrix [M, out_ld bytes] the next E4M3 linear layer reads (fc1 -> fc2).
    * out_ld a multiple of 16 >= 64 ceil(N / 64), out_col0 0, `out` 16-byte aligned, a plain output (no residual, second
    * output, trailing layer or fp32), and block_n 32 only when N <= 32. */
   int32_t a_static;
@@ -183,6 +188,11 @@ int pf_quantize_e4m3_static(int32_t num_src, const void* const* src, const int32
  * swin_layers.py:222,265,428).  rows x C; x_ld/out_ld in elements. */
 int pf_layernorm(const float* x, int32_t x_ld, const float* w, const float* b, float eps, int32_t rows, int32_t C,
                  void* out, int32_t out_ld, void* stream);
+/* pf_layernorm's statistics with an e4m3 output (vit_precision 'fp8_static': the operand of the qkv / fc1 linear):
+ * out[r, c] = e4m3_rn(sat(y * ratio)), y the fp32 affine value (no bf16 rounding in between), ratio = 448 / amax of the
+ * consumer's calibrated input amax (pf_quantize_e4m3_static's rule).  out is [rows, out_ld bytes], out_ld >= C. */
+int pf_layernorm_e4m3(const float* x, int32_t x_ld, const float* w, const float* b, float eps, int32_t rows, int32_t C,
+                      float ratio, void* out, int32_t out_ld, void* stream);
 /* Fused softmax(QK^T * scale) V for the DINOv2 blocks (dinov2/layers/attention.py:49-62): qk is the [B*seq, 2*D]
  * bf16 Q|K part of the qkv GEMM output (row stride qk_ld), vt the transposed V written by pf_gemm;
  * out [B*seq, D] bf16.  head_dim == 64. */
@@ -405,7 +415,9 @@ typedef struct pf_layer {
   /* fusion_precision 'fp8_static': a HOST pointer to the calibrated amax of the conv's input (NULL: per-tile scales as
    * above).  The stage then quantizes the input with pf_quantize_e4m3_static at r = 448 / amax and runs the conv with the
    * static scale amax / 448; the first conv of a U-Net DoubleConv whose second conv is static too writes the second's
-   * e4m3 operand map directly (pf_gemm_desc.out_e4m3).  Read when the stage is issued. */
+   * e4m3 operand map directly (pf_gemm_desc.out_e4m3).  Read when the stage is issued.
+   * vit_precision 'fp8_static': set on a ViT block's qkv, fc1 and fc2 (with w8 / w_scale), the amax of the linear's
+   * input.  LN1 / LN2 then write qkv's / fc1's e4m3 operand (pf_layernorm_e4m3) and fc1 writes fc2's (out_e4m3). */
   const float* a_amax;
 } pf_layer;
 

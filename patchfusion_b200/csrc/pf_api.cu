@@ -581,7 +581,14 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   if (u->out_ld % 8 || u->out_col0 % 8) return set_error("pf_gemm: out_ld/out_col0 must be multiples of 8");
   const bool e4m3 = u->a_e4m3 != 0;
   const bool a_static = e4m3 && u->a_static != 0;
-  if (e4m3 && (u->a_mode != 1 || u->taps != 9 || u->bh != 0 || u->bw != 0 || getenv("PF_B200_NO_HALO") != nullptr ||
+  // a linear layer on e4m3 operands (static scale): pf_gemm_pp_e4m3_kernel
+  const bool lin8 = a_static && u->a_mode == 0 && u->taps == 1;
+  if (lin8 && (u->num_src != 1 || u->N % 128 || u->a_c[0] % 128 || u->a_ld[0] % 16 || u->a_ld[0] < u->a_c[0] || !u->s_w ||
+               u->ps > 1 || u->w2 || u->res1 || u->res2 || u->out2 ||
+               (u->act != PF_ACT_NONE && u->act != PF_ACT_GELU && u->act != PF_ACT_RELU)))
+    return set_error("pf_gemm: an e4m3 linear layer takes one e4m3 matrix source of K (a multiple of 128) <= a_ld "
+                     "(a multiple of 16) byte rows, N a multiple of 128, s_w, and bias -> none / GELU / ReLU into one output");
+  if (e4m3 && !lin8 && (u->a_mode != 1 || u->taps != 9 || u->bh != 0 || u->bw != 0 || getenv("PF_B200_NO_HALO") != nullptr ||
                u->rs_h[0] || u->rs_h[1] || u->rs_h[2] || (!u->s_a && !a_static) || !u->s_w))
     return set_error("pf_gemm: e4m3 operands take the 3x3 halo-tile conv with materialised sources and s_a / s_w");
   if ((u->a_static && !e4m3) || (u->out_e4m3 && !a_static))
@@ -590,8 +597,8 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   const int n_pad64 = (u->N + 63) / 64 * 64;
   if (out8 && (u->out_f32 || u->gamma || u->res1 || u->res2 || u->out2 || u->w2 || u->vt || u->ps > 1 || u->out_col0 ||
                u->out_ld % 16 || u->out_ld < n_pad64 || reinterpret_cast<uintptr_t>(u->out) % 16 || !(u->out_ratio >= 0.f)))
-    return set_error("pf_gemm: an e4m3 output is a plain map of 64 ceil(N / 64) <= out_ld (a multiple of 16) byte rows, "
-                     "16-byte aligned, with out_ratio >= 0");
+    return set_error("pf_gemm: an e4m3 output is a plain map / matrix of 64 ceil(N / 64) <= out_ld (a multiple of 16) "
+                     "byte rows, 16-byte aligned, with out_ratio >= 0");
   GemmDesc d;
   memset(&d, 0, sizeof(d));
   d.num_src = u->num_src; d.a_mode = u->a_mode; d.taps = u->taps;
@@ -671,6 +678,10 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
     d.m_tiles = u->NB * d.tiles_y * d.tiles_x;
     for (int s = 0; s < u->num_src; ++s)
       if (tmap_4d_nhwc_bf16(&tmA[s], u->a_ptr[s], u->a_c[s], u->W, u->H, u->NB, u->a_ld[s], 64, bw, bh)) return 1;
+  } else if (lin8) {
+    // 128-byte K blocks: {128 B, 128 rows} boxes of the e4m3 matrix [M, a_ld[0] bytes]
+    d.m_tiles = (u->M + 127) / 128;
+    if (tmap_2d_u8(&tmA[0], u->a_ptr[0], u->a_c[0], u->M, u->a_ld[0], 128, 128)) return 1;
   } else {
     d.m_tiles = (u->M + 127) / 128;
     for (int s = 0; s < u->num_src; ++s)
@@ -785,7 +796,10 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   if (out8) {
     // the q8 kernel's e4m3 epilogue: {64 bytes, 8 px, 2 rows} boxes of a map N rounded up to 64 columns wide, so the
     // stores write the pad columns (as zero) too
-    if (!no_tma_epi && tmap_4d_nhwc_u8(&tmOut, u->out, n_pad64, u->W, u->H, u->NB, u->out_ld, 64, 8, 2)) return 1;
+    // ({64 bytes, 16 rows} boxes of the linear layer's [M, out_ld bytes] matrix)
+    if (!no_tma_epi && (lin8 ? tmap_2d_u8(&tmOut, u->out, n_pad64, u->M, u->out_ld, 64, 16)
+                             : tmap_4d_nhwc_u8(&tmOut, u->out, n_pad64, u->W, u->H, u->NB, u->out_ld, 64, 8, 2)))
+      return 1;
     d.tma_out = no_tma_epi ? 0 : 1;
   } else if (!no_tma_epi && !(halo && any_rs) && d.ps == 1 && !d.w2 && !d.res1 && !d.res2 && !d.out2 && ends16) {
     // each consumer warp stores its 16 rows in whole column groups (bf16) / 32-column chunks (fp32)
@@ -818,13 +832,23 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
                                static_cast<long long>((u->M + d.vt_seq - 1) / d.vt_seq + 1) * d.vt_dim * d.vt_seq_pad < (1ll << 31));
   if (u->a_mode == 0 && u->num_src == 1 && d.tma_out != 0 && u->N % kPpBN == 0 && bn % kPpBN == 0 && pp_act && pp_vt) {
     d.pp = 1;
-    if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, kPpBN)) return 1;
-    if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, kPpBN / 2)) return 1;
+    const uint64_t rows = static_cast<uint64_t>(d.n_tiles) * bn;
+    if (lin8) {     // the e4m3 panel in 128-byte K blocks, like A
+      if (tmap_2d_u8(&tmB, u->w_ptr, u->Ktot, rows, u->Ktot, 128, kPpBN)) return 1;
+      if (mc && tmap_2d_u8(&tmBh, u->w_ptr, u->Ktot, rows, u->Ktot, 128, kPpBN / 2)) return 1;
+    } else {
+      if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, rows, u->Ktot, 64, kPpBN)) return 1;
+      if (mc && tmap_2d_bf16(&tmBh, u->w_ptr, u->Ktot, rows, u->Ktot, 64, kPpBN / 2)) return 1;
+    }
   }
-  // the FP8 instantiation has only the plain-output fragment epilogue (bias + activation -> stmatrix -> bulk store)
-  if (e4m3 && d.tma_out != 1)
+  // the FP8 conv has only the plain-output fragment epilogue (bias + activation -> stmatrix -> bulk store); the e4m3
+  // linear layer only the ping-pong kernel
+  if (e4m3 && !lin8 && d.tma_out != 1)
     return set_error("pf_gemm: an e4m3 conv needs the bulk-store epilogue: a plain bf16 output, 16-byte aligned, and "
                      "PF_OPT_TMA_EPILOGUE on");
+  if (lin8 && !d.pp)
+    return set_error("pf_gemm: an e4m3 linear layer runs on the ping-pong kernel only: a bulk-store output (16-byte "
+                     "aligned, rows ending on a 16-byte boundary, PF_OPT_TMA_EPILOGUE on)");
   return gemm_launch(d, tmA, tmB, mc ? &tmBh : nullptr, d.tma_out ? &tmOut : nullptr, static_cast<cudaStream_t>(stream));
 }
 

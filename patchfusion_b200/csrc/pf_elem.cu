@@ -59,6 +59,54 @@ __device__ __forceinline__ void ln_row(const float* __restrict__ xr, const float
   }
 }
 
+// pf_layernorm_e4m3: ln_row's statistics, and each fp32 affine value y (the same expression as ln_row's, before any
+// bf16 rounding) written as e4m3_rn(sat(y * ratio)) with cvt.rn.satfinite, four bytes per store
+__device__ __forceinline__ void ln_row_e4m3(const float* __restrict__ xr, const float* __restrict__ w,
+                                            const float* __restrict__ b, float eps, int C, float ratio,
+                                            uint8_t* __restrict__ orow, int lane) {
+  float4 v[8];
+  float s = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    int c = lane * 4 + i * 128;
+    if (c < C) { v[i] = *reinterpret_cast<const float4*>(xr + c); s += v[i].x + v[i].y + v[i].z + v[i].w; }
+  }
+  const float mean = warp_sum(s) / C;
+  float q = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    int c = lane * 4 + i * 128;
+    if (c < C) {
+      float a = v[i].x - mean, bb = v[i].y - mean, cc = v[i].z - mean, d = v[i].w - mean;
+      q += a * a + bb * bb + cc * cc + d * d;
+    }
+  }
+  const float rstd = rsqrtf(warp_sum(q) / C + eps);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    int c = lane * 4 + i * 128;
+    if (c < C) {
+      float4 g = __ldg(reinterpret_cast<const float4*>(w + c));
+      float4 be = __ldg(reinterpret_cast<const float4*>(b + c));
+      const float y0 = (v[i].x - mean) * rstd * g.x + be.x, y1 = (v[i].y - mean) * rstd * g.y + be.y;
+      const float y2 = (v[i].z - mean) * rstd * g.z + be.z, y3 = (v[i].w - mean) * rstd * g.w + be.w;
+      uint16_t lo, hi;
+      asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(lo) : "f"(__fmul_rn(y1, ratio)), "f"(__fmul_rn(y0, ratio)));
+      asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(hi) : "f"(__fmul_rn(y3, ratio)), "f"(__fmul_rn(y2, ratio)));
+      *reinterpret_cast<uint32_t*>(orow + c) = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
+    }
+  }
+}
+__global__ void layernorm_e4m3_kernel(const float* __restrict__ x, int x_ld, const float* __restrict__ w,
+                                      const float* __restrict__ b, float eps, int rows, int C, float ratio,
+                                      uint8_t* __restrict__ out, int out_ld) {
+  pdl_wait();
+  int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  ln_row_e4m3(x + static_cast<long long>(row) * x_ld, w, b, eps, C, ratio, out + static_cast<long long>(row) * out_ld,
+              threadIdx.x & 31);
+}
+
 // rows_out > 0: output row r comes from input row (r / rows_out) * rows_in + skip + r % rows_out (per-image patch
 // tokens with the cls row dropped); rows_out == 0: identity mapping.
 __global__ void layernorm_kernel(const float* __restrict__ x, int x_ld, const float* __restrict__ w,
@@ -1027,6 +1075,18 @@ int pf_layernorm(const float* x, int32_t x_ld, const float* w, const float* b, f
                               static_cast<bf16*>(out), out_ld, 0, 0, 0);
   if (le != cudaSuccess) return set_error("layernorm_kernel launch: %s", cudaGetErrorString(le));
   return check_launch("layernorm_kernel");
+}
+
+int pf_layernorm_e4m3(const float* x, int32_t x_ld, const float* w, const float* b, float eps, int32_t rows, int32_t C,
+                      float ratio, void* out, int32_t out_ld, void* stream) {
+  if (C % 4 || x_ld % 4 || out_ld % 4 || out_ld < C || C > 1024 || rows < 0 || !(ratio >= 0.f) ||
+      reinterpret_cast<uintptr_t>(out) % 4)
+    return set_error("pf_layernorm_e4m3: C (<= 1024) and strides must be multiples of 4, out_ld >= C, out 4-byte "
+                     "aligned, ratio >= 0");
+  cudaError_t le = launch_pdl(layernorm_e4m3_kernel, dim3(nblocks(rows, 8)), dim3(256), 0, ST, x, x_ld, w, b, eps, rows,
+                              C, ratio, static_cast<uint8_t*>(out), out_ld);
+  if (le != cudaSuccess) return set_error("layernorm_e4m3_kernel launch: %s", cudaGetErrorString(le));
+  return check_launch("layernorm_e4m3_kernel");
 }
 
 int pf_layernorm_grouped(const float* x, int32_t x_ld, const float* w, const float* b, float eps, int32_t groups,

@@ -498,21 +498,24 @@ __device__ __forceinline__ void epilogue_tile_tma_bf16(const GemmDesc& d, EpiTma
   }
 }
 
-// e4m3 output (the static-scale halo conv with d.out_e4m3): the dequantized, biased and activated fp32 value v of
-// each element is quantized straight to e4m3_rn(sat(v * out_ratio)), never through bf16, and stored as the operand map
-// of the next E4M3 conv: groups of 64 columns = 64-byte row segments (SWIZZLE_64B: 16-byte piece j of row r at
-// j ^ ((r >> 1) & 3)), one {64 B, 8 px, 2 rows} bulk store per warp and group.  A thread's fragment gives two adjacent
+// e4m3 output (the static-scale halo conv and the E4M3 ping-pong GEMM with d.out_e4m3): the dequantized, biased and
+// activated fp32 value v of each element is quantized straight to e4m3_rn(sat(v * out_ratio)), never through bf16, and
+// stored as the operand of the next E4M3 conv or linear: groups of 64 columns = 64-byte row segments (SWIZZLE_64B:
+// 16-byte piece j of row r at j ^ ((r >> 1) & 3)), one {64 B, 8 px, 2 rows} (conv) or {64 B, 16 rows} (linear) bulk
+// store per warp and group.  A thread's fragment gives two adjacent
 // columns per row and octet, so it writes them as one 16-bit e4m3x2 at byte 32h + 8j + 2 (lane % 4) of rows lane / 4
 // and lane / 4 + 8: per store instruction the eight rows of a warp fall in distinct 16-byte pieces of distinct bank
 // halves, no bank conflict (tests/test_fp8_static_host.py models the layout).  Columns N .. 64 ceil(N / 64) - 1 are
 // written as 0 (the consumer reads whole 64-byte chunks, and a stale byte could be an e4m3 NaN), including the second
-// half of the group at block_n 32 (the host allows that width for N <= 32 only).
+// half of the group at block_n 32 (the host allows that width for N <= 32 only).  FULL (the E4M3 ping-pong GEMM, N a
+// multiple of its 128-column tile): every column of the tile exists, so the column guards go (and with them the
+// registers the multicast instantiation would otherwise spill).
 __device__ __forceinline__ uint32_t e4m3x2_rn(float lo, float hi) {
   uint16_t r;
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
   return r;
 }
-template <int S>
+template <int S, bool FULL = false>
 __device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                        const TileCoord& c, int warp, int lane) {
   constexpr int BN = 2 * S;
@@ -522,7 +525,7 @@ __device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma
   const float rn = d.out_ratio;
   for (int g = 0; 64 * g < (BN < 64 ? 64 : BN); ++g) {
     const int lcol = c.n0 + g * 64;
-    if (lcol >= n_pad) break;
+    if (!FULL && lcol >= n_pad) break;
     const int tile = epi_stage_acquire(e, lane);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -536,7 +539,10 @@ __device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma
       for (int j = 0; j < 4; ++j) {
         const int col = lcol + 32 * h + 8 * j + 2 * q;
         uint32_t lo = 0, hi = 0;
-        if (64 * g + 32 * h < BN) {
+        if (FULL) {
+          lo = e4m3x2_rn(__fmul_rn(v[4 * j], rn), __fmul_rn(v[4 * j + 1], rn));
+          hi = e4m3x2_rn(__fmul_rn(v[4 * j + 2], rn), __fmul_rn(v[4 * j + 3], rn));
+        } else if (64 * g + 32 * h < BN) {
           lo = e4m3x2_rn(col < d.n_logical ? __fmul_rn(v[4 * j], rn) : 0.f,
                          col + 1 < d.n_logical ? __fmul_rn(v[4 * j + 1], rn) : 0.f);
           hi = e4m3x2_rn(col < d.n_logical ? __fmul_rn(v[4 * j + 2], rn) : 0.f,
@@ -563,8 +569,9 @@ __device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma
 // the swizzle; a half-warp's four rows meet in two pieces, a 2-way bank conflict on 8 stores per chunk).
 // The residual-stream update x += gamma * (acc + bias) stages gamma * (acc + bias) and lets the copy engine ADD it into
 // x (cp.reduce.async.bulk.tensor .add.f32, performed in the L2): the SM never reads x.  Each element is updated by
-// exactly one tile: deterministic.
-template <int S>
+// exactly one tile: deterministic.  SC = 2 (the E4M3 ping-pong GEMM): the accumulator is dequantized first, as in
+// epilogue_tile_tma_bf16.
+template <int S, int SC = 0>
 __device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma& e, const float (&acc)[S],
                                                       const TileCoord& c, int warp, int lane) {
   const int r = lane >> 2, q = lane & 3;
@@ -575,6 +582,7 @@ __device__ __forceinline__ void epilogue_tile_tma_f32(const GemmDesc& d, EpiTma&
     const int tile = epi_stage_acquire(e, lane);
     float v[16];
     acc_chunk(ch, acc, v);
+    if constexpr (SC != 0) epi_dequant(d, v, lcol + 2 * q, d.a_scale);
     epi_frag(d, v, lcol + 2 * q, d.gamma != nullptr);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -889,8 +897,8 @@ __device__ __forceinline__ void named_bar_arrive256() { asm volatile("bar.arrive
 // V^T third of a fused qkv projection, stored from the accumulator fragment: vt[(b * heads + h) * 64 + dd][token].
 // For one column the eight lanes 4i + q (i = 0..7) hold eight consecutive tokens, 16 contiguous bytes of a V^T row
 // (split where the tokens cross an image boundary, m / vt_seq).  Same bias -> activation as the row path, so the same
-// bits.  32-bit offsets keep the accumulators' neighbours in registers.
-template <int S>
+// bits.  32-bit offsets keep the accumulators' neighbours in registers.  SC = 2: dequantized first (E4M3 operands).
+template <int S, int SC = 0>
 __device__ __forceinline__ void epilogue_tile_vt(const GemmDesc& d, const float (&acc)[S], const TileCoord& c, int warp,
                                                  int lane) {
   const int q = lane & 3;
@@ -907,6 +915,7 @@ __device__ __forceinline__ void epilogue_tile_vt(const GemmDesc& d, const float 
     if (lcol >= d.n_logical) break;
     float v[16];
     acc_chunk(ch, acc, v);
+    if constexpr (SC != 0) epi_dequant(d, v, lcol + 2 * q, d.a_scale);
     epi_frag(d, v, lcol + 2 * q, false);
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -922,18 +931,34 @@ __device__ __forceinline__ void epilogue_tile_vt(const GemmDesc& d, const float 
   }
 }
 
-// 64 rows x 128 columns of a pf_gemm_pp_kernel tile: rows 16 warp .. 16 warp + 15 of this consumer warp
-template <int S>
+// 64 rows x 128 columns of a pf_gemm_pp_kernel tile: rows 16 warp .. 16 warp + 15 of this consumer warp.  F8 (the E4M3
+// instantiation): every output kind first takes the static-scale dequantization act(fl(acc * fl(a_scale * s_w[n])) +
+// bias[n]) of the q8 halo conv, and d.out_e4m3 adds the e4m3 output (the next linear's operand matrix, 64-byte
+// column groups through a uint8 tensor map: epilogue_tile_tma_e4m3 with {64 B, 16 rows} boxes).
+template <bool F8, int S>
 __device__ __forceinline__ void epilogue_tile_pp(const GemmDesc& d, EpiTma& et, const float (&acc)[S], const TileCoord& c,
                                                  int warp, int lane) {
-  if (d.vt != nullptr && c.n0 >= d.vt_col0) epilogue_tile_vt(d, acc, c, warp, lane);
-  else if (d.tma_out == 2) epilogue_tile_tma_f32(d, et, acc, c, warp, lane);
-  else epilogue_tile_tma_bf16<64>(d, et, acc, c, warp, lane);
+  constexpr int SC = F8 ? 2 : 0;
+  if (d.vt != nullptr && c.n0 >= d.vt_col0) epilogue_tile_vt<S, SC>(d, acc, c, warp, lane);
+  else if (d.tma_out == 2) epilogue_tile_tma_f32<S, SC>(d, et, acc, c, warp, lane);
+  else {
+    if constexpr (F8) {
+      if (d.out_e4m3) {
+        epilogue_tile_tma_e4m3<S, true>(d, et, acc, c, warp, lane);
+        return;
+      }
+    }
+    epilogue_tile_tma_bf16<64, S, SC>(d, et, acc, c, warp, lane);
+  }
 }
 
-template <bool MC>
-__global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __grid_constant__ GemmKernelParams P) {
+// F8: the E4M3 instantiation (pf_gemm_pp_e4m3_kernel, d.a_e4m3 with a static input scale).  A K block is 128 e4m3
+// bytes, so the A and B tiles keep their 128-byte swizzled rows, the 32 KiB stage and the six-stage ring; its four k32
+// steps issue two wgmma.m64n128k32.f32.e4m3.e4m3 each, at the same descriptor offsets as the bf16 k16 steps.
+template <bool MC, bool F8>
+__device__ __forceinline__ void gemm_pp_body(const GemmKernelParams& P) {
   constexpr int CL = MC ? 2 : 1;
+  constexpr int kKBlock = F8 ? 2 * kBlockK : kBlockK;   // K elements of one 128-byte block
   extern __shared__ uint8_t smem_raw[];
   const GemmDesc& d = P.d;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -984,13 +1009,13 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __gri
           uint8_t* sb = sa + kATileBytes;
           if (elect_one()) {
             mbar_expect_tx(&full_bar[stage], kPpStageBytes);
-            tma_load_2d(sa, &P.tmA[0], &full_bar[stage], kb * kBlockK, c.m0);
+            tma_load_2d(sa, &P.tmA[0], &full_bar[stage], kb * kKBlock, c.m0);
             if (MC) {
               constexpr int half_rows = kPpBN / 2;
-              tma_load_2d_mc(sb + it.rank * half_rows * 128, &P.tmBh, &full_bar[stage], kb * kBlockK,
+              tma_load_2d_mc(sb + it.rank * half_rows * 128, &P.tmBh, &full_bar[stage], kb * kKBlock,
                              c.n0 + it.rank * half_rows, static_cast<uint16_t>(3));
             } else {
-              tma_load_2d(sb, &P.tmB, &full_bar[stage], kb * kBlockK, c.n0);
+              tma_load_2d(sb, &P.tmB, &full_bar[stage], kb * kKBlock, c.n0);
             }
           }
           if (++stage == kPpStages) { stage = 0; phase ^= 1; }
@@ -1039,9 +1064,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __gri
         const uint64_t bdesc = wgmma_desc_k128(sa + kATileBytes);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kBlockK / 16; ++k) {
-          Wgmma<kPpBN>::ss(acc0, adesc + 2 * k, bdesc + 2 * k, accum | k);
-          Wgmma<kPpBN>::ss(acc1, adesc1 + 2 * k, bdesc + 2 * k, accum | k);
+        for (int k = 0; k < kBlockK / 16; ++k) {          // 32-byte K steps: k16 bf16 / k32 e4m3
+          if constexpr (F8) {
+            Wgmma8<kPpBN>::ss(acc0, adesc + 2 * k, bdesc + 2 * k, accum | k);
+            Wgmma8<kPpBN>::ss(acc1, adesc1 + 2 * k, bdesc + 2 * k, accum | k);
+          } else {
+            Wgmma<kPpBN>::ss(acc0, adesc + 2 * k, bdesc + 2 * k, accum | k);
+            Wgmma<kPpBN>::ss(acc1, adesc1 + 2 * k, bdesc + 2 * k, accum | k);
+          }
         }
         wgmma_commit();
         accum = 1;
@@ -1059,8 +1089,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __gri
       skip(P.k_steps);                                      // tile p + 1 is the other warpgroup's
       tl.add(2, tl_main);
       const long long tl_epi = tl.now();
-      epilogue_tile_pp(d, et, acc0, c, w, lane);
-      epilogue_tile_pp(d, et, acc1, c, w + 4, lane);
+      epilogue_tile_pp<F8>(d, et, acc0, c, w, lane);
+      epilogue_tile_pp<F8>(d, et, acc1, c, w + 4, lane);
       __syncwarp();
       tl.add(3, tl_epi);
     }
@@ -1070,6 +1100,15 @@ __global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __gri
   }
   __syncthreads();
   if (MC) cluster_sync_all();       // no CTA exits while its peer may still multicast into it / arrive on its barriers
+}
+
+template <bool MC>
+__global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_kernel(const __grid_constant__ GemmKernelParams P) {
+  gemm_pp_body<MC, false>(P);
+}
+template <bool MC>
+__global__ void __launch_bounds__(kGemmThreads, 1) pf_gemm_pp_e4m3_kernel(const __grid_constant__ GemmKernelParams P) {
+  gemm_pp_body<MC, true>(P);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1468,7 +1507,10 @@ static KernelFn gemm_kernel_mc(int bn) {
   }
 }
 static KernelFn gemm_kernel(bool mc, int bn) { return mc ? gemm_kernel_mc<true>(bn) : gemm_kernel_mc<false>(bn); }
-static KernelFn gemm_pp_kernel(bool mc) { return mc ? pf_gemm_pp_kernel<true> : pf_gemm_pp_kernel<false>; }
+static KernelFn gemm_pp_kernel(bool mc, bool f8 = false) {
+  if (f8) return mc ? pf_gemm_pp_e4m3_kernel<true> : pf_gemm_pp_e4m3_kernel<false>;
+  return mc ? pf_gemm_pp_kernel<true> : pf_gemm_pp_kernel<false>;
+}
 
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
                 const CUtensorMap* tmOut, cudaStream_t stream) {
@@ -1480,7 +1522,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       for (int bn : kGemmWidths)
         if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_kernel(mc, bn), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (bool mc : {false, true})
-      if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_pp_kernel(mc), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+      for (bool f8 : {false, true})
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_pp_kernel(mc, f8), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     for (int v = 0; v < 3; ++v)
       for (int cl : {1, 2, 4})
         for (int bn : {32, 64, 128, 192})
@@ -1496,7 +1539,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     int ktrue = 0;
     for (int s = 0; s < d.num_src; ++s) ktrue += d.k_true[s];
     const int n_true = d.ps > 1 ? d.n_logical * d.ps * d.ps : d.N;
-    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? (d.a_static ? (d.out_e4m3 ? "conv3x3_e4m3_static_q8out" : "conv3x3_e4m3_static") : "conv3x3_e4m3") : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : "linear")),
+    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? (d.a_static ? (d.out_e4m3 ? "conv3x3_e4m3_static_q8out" : "conv3x3_e4m3_static") : "conv3x3_e4m3") : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : (d.a_e4m3 ? (d.out_e4m3 ? "linear_e4m3_q8out" : "linear_e4m3") : "linear"))),
               rows, d.taps, ktrue, n_true, d.act ? (d.act == PF_ACT_GELU ? " gelu" : (d.act == PF_ACT_RELU ? " relu" : " softplus")) : "",
               d.gamma ? " gamma" : (d.vt ? " vt" : ""), d.w2 ? " tail" : "");
   }
@@ -1510,6 +1553,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   if (d.tma_out && !tmOut) return set_error("gemm: tma_out without an output tensor map");
   int ks = 0;
   for (int s = 0; s < d.num_src; ++s) ks += d.chunks[s] * d.taps;
+  const bool pp8 = d.pp && d.a_e4m3;
+  if (pp8) ks = d.k_true[0] / (2 * kBlockK);       // 128-byte K blocks of e4m3 (the host checks K % 128 == 0)
   P.k_steps = ks;
   P.total_tiles = d.m_tiles * d.n_tiles;
   if (P.total_tiles <= 0 || ks <= 0) return set_error("gemm: empty problem");
@@ -1559,7 +1604,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   } else {
     if (d.pp && (d.block_n % kPpBN != 0 || d.num_src != 1 || d.a_mode != 0 || !d.tma_out))
       return set_error("gemm: the ping-pong kernel takes plain linear layers at block_n 128 / 256 (block_n %d)", d.block_n);
-    const KernelFn gk = d.pp ? gemm_pp_kernel(tmBh != nullptr) : gemm_kernel(tmBh != nullptr, d.block_n);
+    const KernelFn gk = d.pp ? gemm_pp_kernel(tmBh != nullptr, pp8) : gemm_kernel(tmBh != nullptr, d.block_n);
     if (gk == nullptr) return set_error("gemm: block_n %d (32, 64, 96, 128, 192 or 256)", d.block_n);
     const size_t smem = 1024 + (d.pp ? static_cast<size_t>(kPpStages) * kPpStageBytes
                                      : static_cast<size_t>(gemm_stages(d.block_n)) * gemm_stage_bytes(d.block_n)) +
@@ -1582,12 +1627,14 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
     } else {
       le = launch_pdl(gk, dim3(grid), dim3(kGemmThreads), smem, stream, P);
     }
-    if (le != cudaSuccess) return set_error("%s launch: %s", d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel", cudaGetErrorString(le));
+    if (le != cudaSuccess)
+      return set_error("%s launch: %s", pp8 ? "pf_gemm_pp_e4m3_kernel" : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"),
+                       cudaGetErrorString(le));
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(e));
   count_launch(d.halo ? (d.a_e4m3 ? (d.a_static ? "pf_conv3_halo_e4m3_q8_kernel" : "pf_conv3_halo_e4m3_kernel") : "pf_conv3_halo_kernel")
-                       : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel"));
+                       : (pp8 ? "pf_gemm_pp_e4m3_kernel" : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel")));
   return 0;
 }
 

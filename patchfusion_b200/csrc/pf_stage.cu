@@ -208,6 +208,28 @@ static void conv_static_e4m3(Ctx& c, const pf_layer& L, const void* q, int kc, c
   }
 }
 
+// ---- vit_precision 'fp8_static': a ViT linear layer on the E4M3 ping-pong GEMM (pf_gemm_pp_e4m3_kernel) over the
+// e4m3 matrix A [M, K bytes] at L's static scale; a bf16 / fp32 / gamma / V^T output as `linear`, or, when `next` is
+// given, next's e4m3 operand matrix (out_ld bytes) at next's static ratio.
+static bool vit_block_fp8(const pf_vit_block& b) {
+  return b.qkv.w8 && b.qkv.a_amax && b.fc1.w8 && b.fc1.a_amax && b.fc2.w8 && b.fc2.a_amax;
+}
+static void linear_e4m3(Ctx& c, const pf_layer& L, const void* A, long long M, int K, void* out, int out_f32, int out_ld,
+                        const GemmOpt& o, const pf_layer* next) {
+  if (!c.live()) return;
+  pf_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.num_src = 1; d.a_mode = 0;
+  d.a_ptr[0] = A; d.a_c[0] = K; d.a_ld[0] = K;
+  d.M = static_cast<int32_t>(M);
+  gemm_desc_common(d, L, o, out, out_f32, out_ld);
+  d.w_ptr = L.w8;
+  d.a_e4m3 = 1; d.s_w = L.w_scale;
+  d.a_static = 1; d.a_scale = static_scale(*L.a_amax);
+  if (next != nullptr) { d.out_e4m3 = 1; d.out_ratio = static_ratio(*next->a_amax); }
+  c.chk(pf_gemm(&d, c.stream));
+}
+
 // 3x3 / 1x1 conv over up to three channel-concatenated NHWC sources
 static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_f32, int out_ld,
                       const GemmOpt& o = GemmOpt()) {
@@ -460,23 +482,81 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
                                       static_cast<size_t>(B) * D, static_cast<cudaStream_t>(c.stream));
     if (e != cudaSuccess) c.chk(set_error("cudaMemset2DAsync(vt pad): %s", cudaGetErrorString(e)));
   }
+  // vit_precision 'fp8_static' (blocks whose qkv, fc1 and fc2 carry e4m3 panels and calibrated input amax): the e4m3
+  // operands of qkv / fc1 ([rows, D] bytes, written by LN1 / LN2) and of fc2 ([rows, 4D] bytes, written by fc1).  Only
+  // such a branch allocates them, so the bf16 workspace is what it was.
+  bool any_fp8 = false;
+  for (int i = 0; i < Wb.depth; ++i) any_fp8 = any_fp8 || vit_block_fp8(Wb.blocks[i]);
+  uint8_t* h8 = any_fp8 ? static_cast<uint8_t*>(c.alloc(static_cast<size_t>(rows) * D)) : nullptr;
+  uint8_t* hid8 = any_fp8 ? static_cast<uint8_t*>(c.alloc(static_cast<size_t>(rows) * 4 * D)) : nullptr;
   Map feats[4];
   int nf = 0;
+  char nm[32];
   for (int i = 0; i < Wb.depth; ++i) {
     const pf_vit_block& bw = Wb.blocks[i];
     // x += ls1 * proj(attn(LN(x)));  x += ls2 * fc2(gelu(fc1(LN(x))))   (dinov2/layers/block.py:82-107)
-    if (c.live()) c.chk(pf_layernorm(x, D, bw.n1w, bw.n1b, 1e-6f, static_cast<int32_t>(rows), D, hbuf, D, c.stream));
     GemmOpt oq; oq.vt = vt; oq.vt_col0 = 2 * D; oq.vt_seq = seq; oq.vt_seq_pad = seq_pad;
-    linear(c, bw.qkv, hbuf, rows, D, D, qk, 0, 2 * D, oq);
-    if (c.live()) c.chk(pf_attention(qk, 2 * D, vt, B, seq, seq_pad, Wb.heads, 0.125f, att, D, c.stream));
     GemmOpt o1; o1.gamma = bw.ls1;
-    linear(c, bw.proj, att, rows, D, D, x, 1, D, o1);
-    if (c.live()) c.chk(pf_layernorm(x, D, bw.n2w, bw.n2b, 1e-6f, static_cast<int32_t>(rows), D, hbuf, D, c.stream));
     GemmOpt of; of.act = PF_ACT_GELU;
-    linear(c, bw.fc1, hbuf, rows, D, D, hid, 0, 4 * D, of);
     GemmOpt o2; o2.gamma = bw.ls2;
-    linear(c, bw.fc2, hid, rows, 4 * D, 4 * D, x, 1, D, o2);
-    char nm[16];
+    if (vit_block_fp8(bw)) {
+      // LN1 -> e4m3 at qkv's ratio, qkv on the e4m3 GEMM, attention, proj in bf16 (its input comes from the attention
+      // kernel), LN2 -> e4m3 at fc1's ratio, fc1 + GELU -> fc2's e4m3 operand, fc2 + gamma reduce-add into x.  Debug
+      // taps "e4m3v.<i>.<lin>.in" (the e4m3 operand the linear read) and "e4m3v.<i>.<lin>.out" (what it wrote; qkv's V^T
+      // third is "e4m3v.<i>.qkv.vt", fc2's residual stream before its update "e4m3v.<i>.fc2.x").
+      if (c.live())
+        c.chk(pf_layernorm_e4m3(x, D, bw.n1w, bw.n1b, 1e-6f, static_cast<int32_t>(rows), D, static_ratio(*bw.qkv.a_amax), h8,
+                                D, c.stream));
+      linear_e4m3(c, bw.qkv, h8, rows, D, qk, 0, 2 * D, oq, nullptr);
+      if (c.tap != nullptr) {
+        snprintf(nm, sizeof(nm), "e4m3v.%d.qkv.in", i);
+        c.tap_out(nm, h8, 2, rows, D, D);
+        snprintf(nm, sizeof(nm), "e4m3v.%d.qkv.out", i);
+        c.tap_out(nm, qk, 0, rows, 2 * D, 2 * D);
+        snprintf(nm, sizeof(nm), "e4m3v.%d.qkv.vt", i);
+        c.tap_out(nm, vt, 0, static_cast<long long>(B) * D, seq_pad, seq_pad);
+      }
+      if (c.live()) c.chk(pf_attention(qk, 2 * D, vt, B, seq, seq_pad, Wb.heads, 0.125f, att, D, c.stream));
+      linear(c, bw.proj, att, rows, D, D, x, 1, D, o1);
+      if (c.live())
+        c.chk(pf_layernorm_e4m3(x, D, bw.n2w, bw.n2b, 1e-6f, static_cast<int32_t>(rows), D, static_ratio(*bw.fc1.a_amax), h8,
+                                D, c.stream));
+      linear_e4m3(c, bw.fc1, h8, rows, D, hid8, 0, 4 * D, of, &bw.fc2);
+      if (c.tap != nullptr) {
+        snprintf(nm, sizeof(nm), "e4m3v.%d.fc1.in", i);
+        c.tap_out(nm, h8, 2, rows, D, D);
+        snprintf(nm, sizeof(nm), "e4m3v.%d.fc1.out", i);
+        c.tap_out(nm, hid8, 2, rows, 4 * D, 4 * D);
+        snprintf(nm, sizeof(nm), "e4m3v.%d.fc2.in", i);
+        c.tap_out(nm, hid8, 2, rows, 4 * D, 4 * D);
+        snprintf(nm, sizeof(nm), "e4m3v.%d.fc2.x", i);
+        c.tap_out(nm, x, 1, rows, D, D);
+      }
+      linear_e4m3(c, bw.fc2, hid8, rows, 4 * D, x, 1, D, o2, nullptr);
+      snprintf(nm, sizeof(nm), "e4m3v.%d.fc2.out", i);
+      c.tap_out(nm, x, 1, rows, D, D);
+    } else {
+      // the calibration taps "amaxv.<i>.<lin>": the bf16 inputs of qkv, fc1 and fc2, whose amax 'fp8_static' runs with
+      if (c.live()) c.chk(pf_layernorm(x, D, bw.n1w, bw.n1b, 1e-6f, static_cast<int32_t>(rows), D, hbuf, D, c.stream));
+      if (c.tap != nullptr) {
+        snprintf(nm, sizeof(nm), "amaxv.%d.qkv", i);
+        c.tap_out(nm, hbuf, 0, rows, D, D);
+      }
+      linear(c, bw.qkv, hbuf, rows, D, D, qk, 0, 2 * D, oq);
+      if (c.live()) c.chk(pf_attention(qk, 2 * D, vt, B, seq, seq_pad, Wb.heads, 0.125f, att, D, c.stream));
+      linear(c, bw.proj, att, rows, D, D, x, 1, D, o1);
+      if (c.live()) c.chk(pf_layernorm(x, D, bw.n2w, bw.n2b, 1e-6f, static_cast<int32_t>(rows), D, hbuf, D, c.stream));
+      if (c.tap != nullptr) {
+        snprintf(nm, sizeof(nm), "amaxv.%d.fc1", i);
+        c.tap_out(nm, hbuf, 0, rows, D, D);
+      }
+      linear(c, bw.fc1, hbuf, rows, D, D, hid, 0, 4 * D, of);
+      if (c.tap != nullptr) {
+        snprintf(nm, sizeof(nm), "amaxv.%d.fc2", i);
+        c.tap_out(nm, hid, 0, rows, 4 * D, 4 * D);
+      }
+      linear(c, bw.fc2, hid, rows, 4 * D, 4 * D, x, 1, D, o2);
+    }
     snprintf(nm, sizeof(nm), "block%d", i);
     c.tap_out(nm, x, 1, rows, D, D);
     if (i >= Wb.depth - 4) {

@@ -23,8 +23,8 @@ import torch.nn.functional as F
 
 from . import lib, ops
 from .ops import ACT_GELU, ACT_NONE, ACT_RELU, ACT_SOFTPLUS, call, pad_to, stream_ptr
-from .params import FP8_LAYERS, WINDOW, branch_hparams, fusion_fp8_amax, fusion_precision, guided_fusion_hparams, \
-    normed_attractors, _get
+from .params import FP8_LAYERS, VIT_FP8_LINEARS, WINDOW, branch_hparams, fusion_fp8_amax, fusion_precision, \
+    guided_fusion_hparams, normed_attractors, vit_fp8_amax, vit_fp8_layers, vit_precision, _get
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -68,10 +68,18 @@ class Engine:
         H, W = self.P
         assert H % 14 == 0 and W % 14 == 0
         self.gh, self.gw = H // 14, W // 14
+        # vit_precision 'fp8_static': qkv, fc1 and fc2 of both encoders get e4m3 panels next to their bf16 ones
+        # (calibration runs the bf16 encoder).  c_branch carries the calibrated input amax (set_vit_fp8_amax), c_branch_bf16
+        # is the same stage without them.
+        self.vit_fp8_static = vit_precision(config) == 'fp8_static'
         self.W = {}
         self._pack_all()
         self.sd = None   # fp32 originals are no longer needed on the device
         self.c_branch = {b: self._c_branch(b) for b in ('coarse', 'fine') if b in self.parts}
+        self.c_branch_bf16 = dict(self.c_branch)
+        self.vit_amax = None
+        if self.vit_fp8_static:
+            self.set_vit_fp8_amax(vit_fp8_amax(config))
         self.c_fusion = self._c_fusion() if 'fusion' in self.parts else None
         # 'fp8_static': c_fusion carries the calibrated input amax of each FP8 conv (set_fp8_amax); c_fusion_tiles is the
         # same stage with per-tile scales, which calibration runs.  `calib` (a dict while PatchFusion.calibrate_fp8 runs)
@@ -163,15 +171,19 @@ class Engine:
             pe = torch.cat([pe[:, :1], grid.permute(0, 2, 3, 1).reshape(1, self.gh * self.gw, D)], 1)
         Wd['pos'] = pe[0].contiguous()
         Wd['cls'] = self._f32(vit + 'cls_token').reshape(D)
+
+        def lin(name):      # qkv / fc1 / fc2: e4m3 panels too under vit_precision 'fp8_static'
+            w, b = self._w(name + '.weight'), self._w(name + '.bias')
+            if self.vit_fp8_static:
+                return ops.pack_weight_e4m3(w, b, keep_bf16=True)
+            return ops.pack_weight(w, b)
         for i in range(hp['depth']):
             p = vit + 'blocks.%d.' % i
             Wd['b%d' % i] = dict(
                 n1w=self._f32(p + 'norm1.weight'), n1b=self._f32(p + 'norm1.bias'),
                 n2w=self._f32(p + 'norm2.weight'), n2b=self._f32(p + 'norm2.bias'),
-                qkv=ops.pack_weight(self._w(p + 'attn.qkv.weight'), self._w(p + 'attn.qkv.bias')),
-                proj=ops.pack_weight(self._w(p + 'attn.proj.weight'), self._w(p + 'attn.proj.bias')),
-                fc1=ops.pack_weight(self._w(p + 'mlp.fc1.weight'), self._w(p + 'mlp.fc1.bias')),
-                fc2=ops.pack_weight(self._w(p + 'mlp.fc2.weight'), self._w(p + 'mlp.fc2.bias')),
+                qkv=lin(p + 'attn.qkv'), proj=ops.pack_weight(self._w(p + 'attn.proj.weight'), self._w(p + 'attn.proj.bias')),
+                fc1=lin(p + 'mlp.fc1'), fc2=lin(p + 'mlp.fc2'),
                 ls1=self._f32(p + 'ls1.gamma'), ls2=self._f32(p + 'ls2.gamma'))
         Wd['nw'], Wd['nb'] = self._f32(vit + 'norm.weight'), self._f32(vit + 'norm.bias')
         dh = pre + 'core.core.depth_head.'
@@ -280,7 +292,8 @@ class Engine:
         H.min_depth, H.max_depth = float(_get(depth_cfg, 'min_depth', 1e-3)), float(_get(depth_cfg, 'max_depth', 10))
         return H
 
-    def _c_branch(self, which):
+    def _c_branch(self, which, amax=None):
+        """amax: {'<i>.<qkv|fc1|fc2>': address of its fp32 input amax} of a calibrated 'fp8_static' encoder, or None"""
         from . import stage
         Wd, hp = self.W[which], self.hp[which]
         B = stage.PfBranch()
@@ -297,6 +310,9 @@ class Engine:
                 setattr(cb, k, bw[k].data_ptr())
             for k in ('qkv', 'proj', 'fc1', 'fc2'):
                 setattr(cb, k, stage.layer(bw[k]))
+            if amax is not None:
+                for k in VIT_FP8_LINEARS:
+                    getattr(cb, k).a_amax = amax['%d.%s' % (i, k)]
         self._keep.append(blocks)
         B.blocks = blocks
         B.nw, B.nb = Wd['nw'].data_ptr(), Wd['nb'].data_ptr()
@@ -326,6 +342,30 @@ class Engine:
         self._keep.append(arr)
         self.c_fusion = self._c_fusion({k: ct.addressof(arr) + 4 * i for i, k in enumerate(FP8_LAYERS)})
         self.fp8_amax = table
+
+    def set_vit_fp8_amax(self, table):
+        """vit_precision 'fp8_static': the calibrated input amax of the encoders' qkv / fc1 / fc2 ({name of
+        vit_fp8_layers: float}, validated), or None (no table: the branches refuse to run, calibration still can).  Read
+        when a stage is issued, so graphs captured before a change must be dropped (PatchFusion.engine does)."""
+        if table is None:
+            self.vit_amax, self.c_branch = None, dict(self.c_branch_bf16)
+            return
+        table = dict(table)
+        names = vit_fp8_layers(self.cfg)
+        arr = (ct.c_float * len(names))(*[table[k] for k in names])
+        self._keep.append(arr)
+        addr = {k: ct.addressof(arr) + 4 * i for i, k in enumerate(names)}
+        self.c_branch = {b: self._c_branch(b, {k[len(b) + 1:]: a for k, a in addr.items() if k.startswith(b + '.')})
+                         for b in self.c_branch_bf16}
+        self.vit_amax = table
+
+    def _branch_struct(self, which):
+        if self.calib is not None:
+            return self.c_branch_bf16[which]
+        if self.vit_fp8_static and self.vit_amax is None:
+            raise RuntimeError("vit_precision 'fp8_static' needs the calibrated input scales `vit_fp8_amax`: run "
+                               "PatchFusion.calibrate_fp8 (or tools/calibrate_fp8.py) first")
+        return self.c_branch[which]
 
     def _fusion_struct(self):
         if self.calib is not None:
@@ -396,6 +436,8 @@ class Engine:
     def _tap_cb(self, arena, taps):
         def cb(user, name, ptr, is_f32, rows, cols, ld):
             # is_f32: 0 bf16, 1 fp32, 2 e4m3 bytes (the static FP8 convs' operand maps)
+            if name.startswith(b'amaxv.'):
+                return      # the bf16 encoder's calibration inputs (_calib_vit_cb): not kept
             t = self._view(arena, ptr, (rows, ld), (BF16, F32, torch.uint8)[is_f32])
             taps[name.decode()] = t[:, :cols].clone()
         return cb
@@ -412,13 +454,27 @@ class Engine:
             self.calib[k] = m if k not in self.calib else torch.maximum(self.calib[k], m)
         return cb
 
+    def _calib_vit_cb(self, arena, which):
+        """calibration of the 'fp8_static' encoders: fold the amax of each E4M3 linear's bf16 input (tap
+        "amaxv.<i>.<lin>" of the bf16 stage) into calib['<which>.<i>.<lin>'], NaN-propagating, on the stream the branch
+        is issued on (the current stream, as the launches)"""
+        def cb(user, name, ptr, is_f32, rows, cols, ld):
+            name = name.decode()
+            if not name.startswith('amaxv.'):
+                return
+            lo, hi = torch.aminmax(self._view(arena, ptr, (rows, ld), BF16)[:, :cols])
+            m = torch.maximum(-lo, hi).float()
+            k = '%s.%s' % (which, name[6:])
+            self.calib[k] = m if k not in self.calib else torch.maximum(self.calib[k], m)
+        return cb
+
     # ------------------------------------------------------------------ stages (sequenced inside libpf_b200)
     def branch(self, which, images, taps=None, ws=None):
         """images: planar fp32 [B,3,H,W] in [0,1] (un-normalised).  Returns (depth fp32 [B,H,W], feats[6] Maps
         low->high: x_d0, r4, r3, r2, r1, out_conv) - views into the stage's workspace (`ws`: (arena, byte offset) to
         place it; default = the branch's own arena)."""
         from . import stage
-        cb = self.c_branch[which]
+        cb = self._branch_struct(which)
         B = images.shape[0]
         need = stage.branch_workspace_bytes(cb, B)
         if ws is None:
@@ -427,6 +483,8 @@ class Engine:
             arena, off = ws
         assert images.dtype == F32 and images.is_contiguous() and off % 256 == 0 and off + need <= arena.numel()
         tap = self._tap_cb(arena, taps) if taps is not None else None
+        if tap is None and self.calib is not None and self.vit_fp8_static:
+            tap = self._calib_vit_cb(arena, which)
         out = stage.branch_forward(cb, images, B, arena.data_ptr() + off, need, tap)
         H, W = self.P
         depth = self._view(arena, out.depth, (B, H, W), F32)
@@ -444,7 +502,7 @@ class Engine:
 
     def branch_bytes(self, which, B):
         from . import stage
-        return stage.branch_workspace_bytes(self.c_branch[which], B)
+        return stage.branch_workspace_bytes(self._branch_struct(which), B)
 
     @staticmethod
     def _pf_maps(maps):

@@ -70,6 +70,7 @@ SIGNATURES = {
     'pf_quantize_e4m3_static': [_i, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _i, _i, _i, _f,
                                 _p, _p],
     'pf_layernorm': [_p, _i, _p, _p, _f, _i, _i, _p, _i, _p],
+    'pf_layernorm_e4m3': [_p, _i, _p, _p, _f, _i, _i, _f, _p, _i, _p],
     'pf_layernorm_grouped': [_p, _i, _p, _p, _f, _i, _i, _i, _i, _i, _p, _i, _p],
     'pf_attention': [_p, _i, _p, _i, _i, _i, _i, _f, _p, _i, _p],
     'pf_patch_im2col': [_p, _i, _i, _i, _p, _i, _p],

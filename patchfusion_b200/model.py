@@ -13,7 +13,8 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .params import FP8_LAYERS, ParamTree, _get, fusion_fp8_amax, fusion_precision, state_layout, synthetic_state_dict, relative_position_index
+from .params import FP8_LAYERS, ParamTree, _get, fusion_fp8_amax, fusion_precision, state_layout, synthetic_state_dict, relative_position_index, \
+    vit_fp8_amax, vit_fp8_layers, vit_precision
 
 try:
     from huggingface_hub import PyTorchModelHubMixin
@@ -512,6 +513,8 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             if br.type not in ('ZoeDepth', 'DA-ZoeDepth'):
                 raise NotImplementedError
         self.resizer = Resize(config.patch_process_shape[1], config.patch_process_shape[0])
+        self.vit_precision = vit_precision(config)           # ValueError on anything but 'bf16' / 'fp8_static'
+        vit_fp8_amax(config)                                 # ValueError on a malformed ViT calibration table
         self._build_tree(state_layout(config))      # raises ValueError / NotImplementedError like the reference
         self.consistency_training = False
         self._runtime_init()
@@ -557,26 +560,36 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
                 raise RuntimeError('PatchFusion (H100): the hot path runs on libpf_b200 only; move the model to a '
                                    'CUDA device (there is no CPU fallback)')
             self._engine = Engine(self.config, self.state_dict(), p.device)
-        elif self._engine.fp8_static:
-            # the calibration table is part of the config: a changed table re-points the stage and drops the graphs
+        else:
+            # the calibration tables are part of the config: a changed table re-points the stage and drops the graphs
             # captured with the old scales
-            table = fusion_fp8_amax(self.config)
-            if table != self._engine.fp8_amax:
-                self._engine.set_fp8_amax(table)
-                self._graphs = {}
+            if self._engine.fp8_static:
+                table = fusion_fp8_amax(self.config)
+                if table != self._engine.fp8_amax:
+                    self._engine.set_fp8_amax(table)
+                    self._graphs = {}
+            if self._engine.vit_fp8_static:
+                table = vit_fp8_amax(self.config)
+                if table != self._engine.vit_amax:
+                    self._engine.set_vit_fp8_amax(table)
+                    self._graphs = {}
         return self._engine
 
     @torch.no_grad()
     def calibrate_fp8(self, image_lr, image_hr, cai_mode='m1', process_num=4, tile_cfg=None, reset=False):
-        """Post-training calibration of the static FP8 U-Net ('fp8' and 'fp8_static' models): runs forward(mode='infer')
-        on the given images (the same arguments: batches, mixed geometry, rN modes drawing from `random`) with the
-        per-tile 'fp8' arithmetic on this model's panels, and takes, for each of the 34 FP8 convs, the maximum over all
-        tiles of its input's amax.  That is merged by max into config['fusion_fp8_amax'] (reset=True starts from an
-        empty table), which 'fp8_static' then runs with, and returned.  Runs eagerly: no graph of it is kept, and the
-        graphs of earlier forwards are dropped."""
-        if self.fusion_precision not in ('fp8', 'fp8_static'):
-            raise ValueError("calibrate_fp8 needs fusion_precision 'fp8' or 'fp8_static' (this model: %r)"
-                             % self.fusion_precision)
+        """Post-training calibration of the static FP8 U-Net ('fp8' and 'fp8_static' models) and of the 'fp8_static'
+        ViT encoders: runs forward(mode='infer') on the given images (the same arguments: batches, mixed geometry, rN
+        modes drawing from `random`) with the per-tile 'fp8' U-Net arithmetic and the bf16 encoders on this model's
+        panels, and takes, for each of the 34 FP8 convs and each E4M3 ViT linear, the maximum over all tiles and images
+        of its input's amax.  Each table is merged by max into config['fusion_fp8_amax'] / config['vit_fp8_amax']
+        (reset=True starts from empty tables), which 'fp8_static' then runs with.  Returns the U-Net table, or the ViT
+        table when the U-Net is not FP8.  Runs eagerly: no graph of it is kept, and the graphs of earlier forwards are
+        dropped."""
+        unet = self.fusion_precision in ('fp8', 'fp8_static')
+        vit = self.vit_precision == 'fp8_static'
+        if not unet and not vit:
+            raise ValueError("calibrate_fp8 needs fusion_precision 'fp8' or 'fp8_static', or vit_precision 'fp8_static' "
+                             "(this model: %r, %r)" % (self.fusion_precision, self.vit_precision))
         eng = self.engine()
         eng.calib = {}
         graphs, self.use_cuda_graphs = self.use_cuda_graphs, False
@@ -587,19 +600,24 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             eng.calib = None
             self.use_cuda_graphs = graphs
             self._graphs = {}
-        missing = [k for k in FP8_LAYERS if k not in found]
-        if missing:
-            raise RuntimeError('calibrate_fp8: no input amax for %s (a conv read through PF_OPT_FUSED_RESAMPLE has no '
-                               'materialised input to measure)' % missing)
-        table = {} if reset else dict(fusion_fp8_amax(self.config) or {})
-        for k in FP8_LAYERS:
-            table[k] = max(table.get(k, 0.0), found[k]) if found[k] == found[k] else found[k]
-        self.config['fusion_fp8_amax'] = fusion_fp8_amax(dict(fusion_fp8_amax=table))   # ValueError on NaN / inf
         hub = getattr(self, '_hub_mixin_config', None)
-        if isinstance(hub, dict):                   # the config save_pretrained writes
-            hub['fusion_fp8_amax'] = dict(self.config['fusion_fp8_amax'])
+        for on, key, names, check in ((unet, 'fusion_fp8_amax', FP8_LAYERS, fusion_fp8_amax),
+                                      (vit, 'vit_fp8_amax', vit_fp8_layers(self.config), vit_fp8_amax)):
+            if not on:
+                continue
+            missing = [k for k in names if k not in found]
+            if missing:
+                raise RuntimeError('calibrate_fp8: no input amax for %s (a conv read through PF_OPT_FUSED_RESAMPLE has '
+                                   'no materialised input to measure)' % missing)
+            table = {} if reset else dict(check(self.config) or {})
+            for k in names:
+                table[k] = max(table.get(k, 0.0), found[k]) if found[k] == found[k] else found[k]
+            self.config[key] = check({key: table, 'coarse_branch': self.config.coarse_branch,
+                                      'fine_branch': self.config.fine_branch})     # ValueError on NaN / inf
+            if isinstance(hub, dict):               # the config save_pretrained writes
+                hub[key] = dict(self.config[key])
         self.engine()
-        return dict(self.config['fusion_fp8_amax'])
+        return dict(self.config['fusion_fp8_amax'] if unet else self.config['vit_fp8_amax'])
 
     def invalidate(self):
         super().invalidate()

@@ -269,6 +269,40 @@ def gemm(pw, srcs, out, *, image=None, ps_image=None, M=None, act=ACT_NONE, res1
     return d
 
 
+def linear_e4m3(pw, q, amax, out, act=ACT_NONE, out_f32=False, gamma=None, vt=None, out_amax=None, block_n=0):
+    """The E4M3 ping-pong GEMM (pf_gemm_pp_e4m3_kernel) over q, an e4m3 matrix [M, K] (uint8 storage) quantized at the
+    static ratio of `amax`, with pw from pack_weight_e4m3.  out: bf16 [M, ld] (vt = (buffer [B*D_v, seq_pad], vt_col0,
+    seq): the fused qkv projection's V^T third), fp32 [M, ld] (gamma: out += gamma * v), or, with out_amax, the e4m3
+    matrix [M, ld bytes] of the next linear at that amax's ratio."""
+    M, K = q.shape
+    assert q.dtype == torch.uint8 and pw.taps == 1 and pw.Ktot == K
+    d = GemmDesc()
+    d.num_src, d.taps, d.a_mode = 1, 1, 0
+    d.a_ptr[0], d.a_c[0], d.a_ld[0] = q.data_ptr(), K, q.stride(0)
+    d.M = M
+    d.w_ptr = pw.w8.data_ptr()
+    d.N, d.Ktot, d.block_n = pw.N, pw.Ktot, block_n
+    d.bias = pw.bias.data_ptr() if pw.bias is not None else None
+    d.act = act
+    d.out, d.out_ld = out.data_ptr(), out.stride(0)
+    d.out_f32 = 1 if out_f32 or gamma is not None else 0
+    d.gamma = gamma.data_ptr() if gamma is not None else None
+    if vt is not None:
+        vbuf, d.vt_col0, d.vt_seq = vt
+        d.vt, d.vt_seq_pad, d.vt_dim = vbuf.data_ptr(), vbuf.shape[-1], pw.N - d.vt_col0
+    d.a_e4m3, d.a_static, d.a_scale, d.s_w = 1, 1, e4m3_static_scale(amax), pw.w_scale.data_ptr()
+    if out_amax is not None:
+        d.out_e4m3, d.out_ratio = 1, e4m3_static_ratio(out_amax)
+    call('pf_gemm', C.byref(d), stream_ptr())
+    return d
+
+
+def layernorm_e4m3(x, w, b, eps, amax, out):
+    """pf_layernorm_e4m3: LayerNorm of fp32 x [rows, ld] into the e4m3 matrix out [rows, ld bytes] at amax's ratio"""
+    call('pf_layernorm_e4m3', x, x.stride(0), w, b, C.c_float(eps), x.shape[0], w.shape[0], C.c_float(e4m3_static_ratio(amax)),
+         out, out.stride(0), stream_ptr())
+
+
 def gemm_convT(pw, src, image, out):
     """ConvTranspose k==s: src [NB*H*W, ld] rows in (n,y,x) order, out NHWC [NB, H*k, W*k, ld_out]."""
     return gemm(pw, [src], out, ps_image=image, M=image[0] * image[1] * image[2])

@@ -78,6 +78,53 @@ def fusion_fp8_amax(config):
     return out
 
 
+VIT_PRECISIONS = ('bf16', 'fp8_static')
+# The ViT linears that run E4M3 under vit_precision 'fp8_static', per block of each branch's encoder
+VIT_FP8_LINEARS = ('qkv', 'fc1', 'fc2')
+
+
+def vit_precision(config):
+    """Top-level `vit_precision`: what the qkv, fc1 and fc2 linears of both branches' DINOv2 encoders compute in.
+    'bf16' (default), or 'fp8_static': E4M3 operands with one calibrated scale per linear input (`vit_fp8_amax`,
+    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision."""
+    p = _get(config, 'vit_precision', 'bf16')
+    if p not in VIT_PRECISIONS:
+        raise ValueError("vit_precision should be one of 'bf16', 'fp8_static'")
+    return p
+
+
+def vit_fp8_layers(config):
+    """The names of vit_fp8_amax: '{coarse|fine}.{i}.{qkv|fc1|fc2}' for every block i of each branch's encoder"""
+    names = []
+    for b in ('coarse', 'fine'):
+        depth = branch_hparams(_get(config, b + '_branch'))['depth']
+        names += ['%s.%d.%s' % (b, i, k) for i in range(depth) for k in VIT_FP8_LINEARS]
+    return tuple(names)
+
+
+def vit_fp8_amax(config):
+    """Top-level `vit_fp8_amax`: the calibrated amax of each E4M3 ViT linear's input, {name of vit_fp8_layers: float
+    >= 0} with exactly those 6 * depth names, or None when the config has no table.  Anything else raises ValueError."""
+    t = _get(config, 'vit_fp8_amax', None)
+    if t is None:
+        return None
+    names = vit_fp8_layers(config)
+    if not isinstance(t, dict):
+        raise ValueError('vit_fp8_amax should be a dict of the %d ViT linear names to their input amax' % len(names))
+    known = set(names)
+    missing = [k for k in names if k not in t]
+    unknown = sorted(str(k) for k in t if k not in known)
+    if missing or unknown:
+        raise ValueError('vit_fp8_amax: missing layers %s, unknown layers %s' % (missing, unknown))
+    out = {}
+    for k in names:
+        v = t[k]
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
+            raise ValueError('vit_fp8_amax[%r] = %r: a finite float >= 0 is required' % (k, v))
+        out[k] = float(v)
+    return out
+
+
 def branch_hparams(branch_cfg):
     enc = _get(branch_cfg, 'midas_model_type')
     if enc not in ENCODERS:
