@@ -135,6 +135,15 @@ typedef struct pf_gemm_desc {
   float a_scale;
   int32_t out_e4m3;
   float out_ratio;
+  /* Residuals and an e4m3 ReLU copy on a static-scale E4M3 3x3 conv (dpt_precision 'fp8_static': the DPT decoder's
+   * ResidualConvUnits and reassemble convs; pf_conv3_halo_e4m3_res_kernel): with a_static set and a bf16 `out`,
+   * res1 / res2 (bf16, even res_ld >= N, 4-byte aligned) are added as in the bf16 path, v = act(fl(acc * fl(a_scale *
+   * s_w[n])) + bias[n]), then + res1, then + res2 in fp32, and out2_e4m3 != 0 makes out2 an e4m3 NHWC map [NB, H, W,
+   * out2_ld bytes] that receives q = e4m3_rn(sat(max(bf16(v), 0) * out2_ratio)), quantized from the bf16-rounded output
+   * (so q is pf_quantize_e4m3_static of the output's ReLU at r = out2_ratio), columns N .. 64 ceil(N / 64) - 1 zero.
+   * out2_ld a multiple of 16 >= 64 ceil(N / 64), out2 16-byte aligned, out_col0 0, block_n 0, 64 or 128. */
+  int32_t out2_e4m3;
+  float out2_ratio;
 } pf_gemm_desc;
 
 int pf_gemm(pf_gemm_desc* desc, void* stream);

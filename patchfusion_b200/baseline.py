@@ -28,13 +28,14 @@ def _attr(cfg):
 class BaselinePretrain(TiledModel):
     def __init__(self, coarse_branch, fine_branch, sigloss, min_depth, max_depth, image_raw_shape=(2160, 3840),
                  patch_process_shape=(384, 512), patch_split_num=(4, 4), target='coarse', coarse_branch_zoe=None,
-                 fusion_precision=None, fusion_fp8_amax=None, vit_precision=None, vit_fp8_amax=None):
+                 fusion_precision=None, fusion_fp8_amax=None, vit_precision=None, vit_fp8_amax=None,
+                 dpt_precision=None, dpt_fp8_amax=None):
         nn.Module.__init__(self)
         # fusion_precision selects the compute type of PatchFusion's Guided-Fusion U-Net and fusion_fp8_amax holds its
         # calibrated FP8 input scales; this model has no fusion stage, so a config that carries the keys (any value)
-        # builds and packs exactly as without them.  vit_precision / vit_fp8_amax (PatchFusion's FP8 ViT encoders) are
-        # ignored the same way: FP8 baselines are not built.
-        del fusion_precision, fusion_fp8_amax, vit_precision, vit_fp8_amax
+        # builds and packs exactly as without them.  vit_precision / vit_fp8_amax and dpt_precision / dpt_fp8_amax
+        # (PatchFusion's FP8 ViT encoders and DPT decoders) are ignored the same way: FP8 baselines are not built.
+        del fusion_precision, fusion_fp8_amax, vit_precision, vit_fp8_amax, dpt_precision, dpt_fp8_amax
         # patch_process_shape is deliberately not checked against the 14-px patch here: the shipped coarse configs
         # keep the (384, 512) default, and the reference fails only when a forward runs at a non-multiple of 14
         self.patch_process_shape = tuple(patch_process_shape)

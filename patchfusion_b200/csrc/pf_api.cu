@@ -599,6 +599,19 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
                u->out_ld % 16 || u->out_ld < n_pad64 || reinterpret_cast<uintptr_t>(u->out) % 16 || !(u->out_ratio >= 0.f)))
     return set_error("pf_gemm: an e4m3 output is a plain map / matrix of 64 ceil(N / 64) <= out_ld (a multiple of 16) "
                      "byte rows, 16-byte aligned, with out_ratio >= 0");
+  // residuals and / or an e4m3 ReLU copy on a static-scale E4M3 conv: pf_conv3_halo_e4m3_res_kernel
+  const bool copy8 = u->out2_e4m3 != 0;
+  const bool res8 = a_static && !lin8 && (copy8 || u->res1 || u->res2);
+  if (copy8 && !res8) return set_error("pf_gemm: an e4m3 ReLU copy (out2_e4m3) needs a static-scale E4M3 3x3 conv");
+  if (res8 && (out8 || u->out_f32 || u->gamma || u->w2 || u->vt || u->ps > 1 || u->out_col0 || !u->out2 != !copy8 ||
+               (u->block_n != 0 && u->block_n != 64 && u->block_n != 128) ||
+               ((u->res1 || u->res2) && (u->res_ld % 2 || u->res_ld < u->N ||
+                                         (reinterpret_cast<uintptr_t>(u->res1) | reinterpret_cast<uintptr_t>(u->res2)) % 4)) ||
+               (copy8 && (u->out2_ld % 16 || u->out2_ld < n_pad64 || reinterpret_cast<uintptr_t>(u->out2) % 16 ||
+                          !(u->out2_ratio >= 0.f)))))
+    return set_error("pf_gemm: residuals / an e4m3 ReLU copy on an e4m3 conv take a bf16 output at column 0, block_n 0, "
+                     "64 or 128, bf16 residuals of an even pitch >= N, and an e4m3 copy map of 64 ceil(N / 64) <= out2_ld "
+                     "(a multiple of 16) byte rows, 16-byte aligned, with out2_ratio >= 0");
   GemmDesc d;
   memset(&d, 0, sizeof(d));
   d.num_src = u->num_src; d.a_mode = u->a_mode; d.taps = u->taps;
@@ -718,7 +731,11 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   // such a conv takes 64-column n-tiles even where the panel's n_pad rows are a multiple of 32 only (N = 160 in the
   // vits U-Net): its weight maps then end at n_pad rows and the copy engine zero-fills the rows past them.
   uint64_t b_rows = 0;
-  if (out8 && bn == 32 && u->N > 32) {
+  if (res8) {
+    // the kernel's widths are 64 and 128; a last n-tile past the panel's n_pad rows reads the copy engine's zero fill
+    if (u->block_n == 0) bn = n_pad % 128 == 0 ? 128 : 64;
+    b_rows = static_cast<uint64_t>(n_pad);
+  } else if (out8 && bn == 32 && u->N > 32) {
     if (u->block_n != 0) return set_error("pf_gemm: an e4m3 output needs block_n >= 64 when N > 32 (N %d)", u->N);
     bn = 64;
     b_rows = static_cast<uint64_t>(n_pad);
@@ -730,7 +747,7 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
     if (tmap_2d_u8(&tmB, u->w_ptr, u->Ktot, b_rows, u->Ktot, 64, bn)) return 1;
     d.a_e4m3 = 1; d.s_a = u->s_a; d.s_w = u->s_w;
     d.a_static = a_static ? 1 : 0; d.a_scale = u->a_scale;
-    d.out_e4m3 = out8 ? 1 : 0; d.out_ratio = u->out_ratio;
+    d.out_e4m3 = out8 ? 1 : 0; d.out_ratio = copy8 ? u->out2_ratio : u->out_ratio;
   } else if (tmap_2d_bf16(&tmB, u->w_ptr, u->Ktot, static_cast<uint64_t>(d.n_tiles) * bn, u->Ktot, 64, bn)) {
     return 1;
   }
@@ -787,13 +804,23 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   // chunks.  Halo convs reading a fused resample keep the direct stores.  PF_OPT_TMA_EPILOGUE = 0 keeps the direct
   // stores everywhere.
   const bool no_tma_epi = option(PF_OPT_TMA_EPILOGUE) == 0;
-  CUtensorMap tmOut;
+  CUtensorMap tmOut, tmOut2;
   d.tma_out = 0;
   // The copy clips columns >= out_col0 + N only at 16-byte granularity: a row that ends inside a 16-byte piece would get
   // the staged zeros of columns N .. written over what the caller keeps there, so such outputs take the direct stores.
   const uint64_t ocols = static_cast<uint64_t>(u->out_col0) + u->N;
   const bool ends16 = ocols % (d.out_f32 ? 4 : 8) == 0;
-  if (out8) {
+  if (res8) {
+    // the bf16 output in {64 ch, 8 px, 2 rows} boxes as a plain halo conv's, the e4m3 copy as the q8 kernel's e4m3 map
+    if (!no_tma_epi) {
+      if (!ends16 || reinterpret_cast<uintptr_t>(u->out) % 16)
+        return set_error("pf_gemm: an e4m3 conv with residuals / a ReLU copy needs a 16-byte aligned bf16 output whose rows end "
+                         "on a 16-byte boundary");
+      if (tmap_4d_nhwc_bf16(&tmOut, u->out, ocols, u->W, u->H, u->NB, u->out_ld, 64, 8, 2)) return 1;
+      if (copy8 && tmap_4d_nhwc_u8(&tmOut2, u->out2, n_pad64, u->W, u->H, u->NB, u->out2_ld, 64, 8, 2)) return 1;
+      d.tma_out = 1;
+    }
+  } else if (out8) {
     // the q8 kernel's e4m3 epilogue: {64 bytes, 8 px, 2 rows} boxes of a map N rounded up to 64 columns wide, so the
     // stores write the pad columns (as zero) too
     // ({64 bytes, 16 rows} boxes of the linear layer's [M, out_ld bytes] matrix)
@@ -849,7 +876,8 @@ int pf_gemm(pf_gemm_desc* u, void* stream) {
   if (lin8 && !d.pp)
     return set_error("pf_gemm: an e4m3 linear layer runs on the ping-pong kernel only: a bulk-store output (16-byte "
                      "aligned, rows ending on a 16-byte boundary, PF_OPT_TMA_EPILOGUE on)");
-  return gemm_launch(d, tmA, tmB, mc ? &tmBh : nullptr, d.tma_out ? &tmOut : nullptr, static_cast<cudaStream_t>(stream));
+  return gemm_launch(d, tmA, tmB, mc ? &tmBh : nullptr, d.tma_out ? &tmOut : nullptr, static_cast<cudaStream_t>(stream),
+                     res8 && copy8 && d.tma_out ? &tmOut2 : nullptr);
 }
 
 }  // extern "C"

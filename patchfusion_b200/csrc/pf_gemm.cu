@@ -74,6 +74,9 @@ struct GemmKernelParams {
   GemmDesc d;
   int total_tiles;
   int k_steps;  // 64-wide K blocks per tile
+  // pf_conv3_halo_e4m3_res_kernel: the e4m3 ReLU copy d.out2 ({64 B, 8 px, 2 rows} boxes).  Last, so that the other
+  // kernels' parameter offsets are what they were.
+  CUtensorMap tmOut2;
 };
 
 
@@ -559,6 +562,122 @@ __device__ __forceinline__ void epilogue_tile_tma_e4m3(const GemmDesc& d, EpiTma
     __syncwarp();
     if (lane == 0) {
       epi_tma_store(d, e, e.stg_ptr + tile, c, warp, lcol);
+      bulk_commit();
+    }
+  }
+}
+
+// pf_conv3_halo_e4m3_res_kernel (the DPT decoder's convs under dpt_precision 'fp8_static'): the static-scale bf16
+// epilogue of the q8 kernel, v = act(fl(acc * fl(a_scale * s_w[n])) + bias[n]), then + res1, then + res2 in fp32 (the
+// order of the row-per-thread epilogue), stored as bf16 through stmatrix staging and {64 ch, 8 px, 2 rows} bulk stores.
+// The residuals are read in the fragment layout straight from global memory: a thread's two adjacent columns of one
+// pixel are one 4-byte bf16x2 load, and the four lanes of a pixel read 16 contiguous bytes.  Every residual element is
+// read exactly once, so staging it through shared memory (a TMA load, then ldmatrix) would add a barrier round trip and
+// a second pass over shared memory for no reuse; the loads of a 32-column chunk are all issued before the first add.
+// Pixels past W / H (and a cluster's phantom tile) read nothing; the bulk store clips them.
+// d.out2 != nullptr adds the e4m3 ReLU copy q = e4m3_rn(sat(max(bf16(v), 0) * d.out_ratio)): quantized from the
+// bf16-ROUNDED value, so it equals pf_quantize_e4m3_static of the bf16 output's ReLU element for element.  It is the
+// q8 kernel's e4m3 output (64-byte SWIZZLE_64B staging tile, e4m3x2 stores, pad columns up to 64 ceil(N / 64) zero)
+// in the warp's second staging tile (the bf16 values go to the first), stored through P.tmOut2 after the group's bf16
+// store.
+__device__ __forceinline__ float2 res_pair(const __nv_bfloat16* row, int col, int n) {
+  if (col + 1 < n) return __bfloat1622float2(__ldg(reinterpret_cast<const __nv_bfloat162*>(row + col)));
+  return make_float2(col < n ? __bfloat162float(row[col]) : 0.f, 0.f);
+}
+template <int S>
+__device__ __forceinline__ void epilogue_tile_tma_res(const GemmDesc& d, EpiTma& e, const CUtensorMap* tm2,
+                                                      const float (&acc)[S], const TileCoord& c, int warp, int lane) {
+  constexpr int BN = 2 * S;
+  static_assert(BN % 64 == 0, "whole 64-column groups");
+  const int r0 = lane >> 2, q = lane & 3;
+  // this thread's pixels: tile rows 16 warp + r0 and + 8 of the 16 x 8 pixel tile = (y0 + 2 warp + i, x0 + r0)
+  const __nv_bfloat16* rrow[2][2];          // [residual][pixel], nullptr: no such residual or pixel
+  {
+    const int x = c.x0 + r0;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int y = c.y0 + 2 * warp + i;
+      const bool ok = c.img < d.NB && y < d.H && x < d.W;
+      const long long pix = (static_cast<long long>(c.img) * d.H + y) * d.W + x;
+      rrow[0][i] = ok && d.res1 != nullptr ? d.res1 + pix * d.res_ld : nullptr;
+      rrow[1][i] = ok && d.res2 != nullptr ? d.res2 + pix * d.res_ld : nullptr;
+    }
+  }
+  const int oct = lane >> 4;
+  const uint32_t lane_off = (lane & 15) * 128;
+  const int swz = lane & 7;
+  const uint32_t swz8 = (r0 >> 1) & 3;
+  const float rn = d.out_ratio;
+  const bool copy = d.out2 != nullptr;
+  const int n = d.n_logical;
+  const int n_pad = (n + 63) & ~63;
+  for (int g = 0; 64 * g < BN; ++g) {
+    const int lcol = c.n0 + g * 64;
+    if (lcol >= n_pad) break;             // (lcol is a multiple of 64: lcol < n_pad means lcol < N)
+    // with the copy, the group's bf16 tile and copy tile are both filled in one pass: wait until the bulk stores of
+    // the previous group have read both (the copy's bytes are then written as they are made, not held in registers)
+    int tile = 0;
+    if (copy) {
+      if (lane == 0) bulk_wait_read0();
+      __syncwarp();
+    } else {
+      tile = epi_stage_acquire(e, lane);
+    }
+    uint8_t* t8 = e.stg_ptr + kXposeWarp;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int col0 = lcol + 32 * h + 2 * q;
+      uint32_t rv[2][2][4];                 // the residuals' bf16x2 pairs
+#pragma unroll
+      for (int r = 0; r < 2; ++r)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 t = rrow[r][i] != nullptr ? res_pair(rrow[r][i], col0 + 8 * j, n) : make_float2(0.f, 0.f);
+            rv[r][i][j] = pack_bf16(t.x, t.y);
+          }
+      float v[16];
+      acc_chunk(2 * g + h, acc, v);
+      epi_dequant(d, v, col0, d.a_scale);
+      epi_frag(d, v, col0, false);
+      uint32_t pk[4][2];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float lo = v[4 * j + 2 * i], hi = v[4 * j + 2 * i + 1];
+#pragma unroll
+          for (int r = 0; r < 2; ++r)
+            if (rrow[r][i] != nullptr) {
+              const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&rv[r][i][j]));
+              lo += t.x; hi += t.y;
+            }
+          pk[j][i] = pack_bf16(lo, hi);
+          if (copy) {
+            const int col = col0 + 8 * j;
+            const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&pk[j][i]));
+            const int by = 32 * h + 8 * j + 2 * q;  // byte within the 64-byte row segment
+            const uint32_t off = static_cast<uint32_t>((((by >> 4) ^ swz8) << 4) | (by & 15));
+            *reinterpret_cast<uint16_t*>(t8 + (r0 + 8 * i) * 64 + off) = static_cast<uint16_t>(
+                e4m3x2_rn(col < n ? __fmul_rn(fmaxf(b.x, 0.f), rn) : 0.f, col + 1 < n ? __fmul_rn(fmaxf(b.y, 0.f), rn) : 0.f));
+          }
+        }
+#pragma unroll
+      for (int p = 0; p < 2; ++p) {
+        const int o = 4 * h + 2 * p;           // octets o (lanes 0-15) and o + 1 (lanes 16-31)
+        const uint32_t addr = e.stg + tile + lane_off + (((o + oct) ^ swz) << 4);
+        stmatrix_x4(addr, pk[2 * p][0], pk[2 * p][1], pk[2 * p + 1][0], pk[2 * p + 1][1]);
+      }
+    }
+    fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      epi_tma_store(d, e, e.stg_ptr + tile, c, warp, d.out_col0 + lcol);
+      bulk_commit();
+    }
+    if (copy && lane == 0) {
+      tma_store_4d(tm2, t8, lcol, c.x0, c.y0 + 2 * warp, c.img);
       bulk_commit();
     }
   }
@@ -1245,7 +1364,9 @@ __device__ __forceinline__ void halo_a_frags(uint32_t ra, int lane, uint32_t (&f
 //
 // Q8 (F8 only): the static-scale instantiation (pf_conv3_halo_e4m3_q8_kernel, d.a_static): one input scale d.a_scale
 // for the launch, and either the bf16 output or (d.out_e4m3) the e4m3 operand map of the next conv.
-template <int CL, int BN, bool F8, bool Q8 = false>
+// RES (Q8 only): pf_conv3_halo_e4m3_res_kernel, the bf16 output with residuals and the e4m3 ReLU copy
+// (epilogue_tile_tma_res).
+template <int CL, int BN, bool F8, bool Q8 = false, bool RES = false>
 __device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
   constexpr bool MC = CL > 1;
   constexpr uint16_t kMask = static_cast<uint16_t>((1u << CL) - 1);
@@ -1279,6 +1400,7 @@ __device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
     // a multicast weight stage is refilled only after the consumers of ALL CTAs of the cluster released it
     for (int s = 0; s < stages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], kEpiWarps * CL); }
     if (d.tma_out) prefetch_tmap(&P.tmOut);
+    if (RES && d.out2 != nullptr) prefetch_tmap(&P.tmOut2);
     fence_barrier_init();
   }
   __syncthreads();
@@ -1426,7 +1548,9 @@ __device__ __forceinline__ void conv3_halo_body(const GemmKernelParams& P) {
       // plain bf16 outputs (the host sets tma_out for the whole launch): fragment layout, stmatrix staging, bulk
       // stores of {G ch, 8 px, 2 rows} boxes (TMA clips pixels past W / H, columns past the output and the phantom
       // img >= NB tile of a cluster); everything else row per thread
-      if constexpr (Q8) {
+      if constexpr (RES) {
+        epilogue_tile_tma_res(d, et, &P.tmOut2, acc, c, warp, lane);
+      } else if constexpr (Q8) {
         if (d.out_e4m3) epilogue_tile_tma_e4m3(d, et, acc, c, warp, lane);
         else epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, 2>(d, et, acc, c, warp, lane);
       } else if constexpr (F8) epilogue_tile_tma_bf16<BN == 32 ? 32 : 64, BN / 2, 1>(d, et, acc, c, warp, lane);
@@ -1454,6 +1578,10 @@ __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_kernel(con
 template <int CL, int BN>
 __global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_q8_kernel(const __grid_constant__ GemmKernelParams P) {
   conv3_halo_body<CL, BN, true, true>(P);
+}
+template <int CL, int BN>
+__global__ void __launch_bounds__(kHaloThreads, 1) pf_conv3_halo_e4m3_res_kernel(const __grid_constant__ GemmKernelParams P) {
+  conv3_halo_body<CL, BN, true, true, true>(P);
 }
 
 
@@ -1484,12 +1612,22 @@ static KernelFn halo_q8_kernel_cl(int bn) {
     default: return nullptr;
   }
 }
+// the DPT decoder's widths: N = C = 64 / 128 / 256 (two 128-column n-tiles) and output_conv1's C / 2 = 64 / 128
+template <int CL>
+static KernelFn halo_res_kernel_cl(int bn) {
+  switch (bn) {
+    case 64: return pf_conv3_halo_e4m3_res_kernel<CL, 64>;
+    case 128: return pf_conv3_halo_e4m3_res_kernel<CL, 128>;
+    default: return nullptr;
+  }
+}
 template <bool F8>
 static KernelFn halo_kernel_t(int cl, int bn) {
   return cl == 4 ? halo_kernel_cl<4, F8>(bn) : (cl == 2 ? halo_kernel_cl<2, F8>(bn) : halo_kernel_cl<1, F8>(bn));
 }
-// q8: pf_conv3_halo_e4m3_q8_kernel (static input scale), f8 must be set too
-static KernelFn halo_kernel(int cl, int bn, bool f8 = false, bool q8 = false) {
+// q8: pf_conv3_halo_e4m3_q8_kernel (static input scale), f8 must be set too; res: pf_conv3_halo_e4m3_res_kernel, q8 too
+static KernelFn halo_kernel(int cl, int bn, bool f8 = false, bool q8 = false, bool res = false) {
+  if (res) return cl == 4 ? halo_res_kernel_cl<4>(bn) : (cl == 2 ? halo_res_kernel_cl<2>(bn) : halo_res_kernel_cl<1>(bn));
   if (q8) return cl == 4 ? halo_q8_kernel_cl<4>(bn) : (cl == 2 ? halo_q8_kernel_cl<2>(bn) : halo_q8_kernel_cl<1>(bn));
   return f8 ? halo_kernel_t<true>(cl, bn) : halo_kernel_t<false>(cl, bn);
 }
@@ -1513,7 +1651,7 @@ static KernelFn gemm_pp_kernel(bool mc, bool f8 = false) {
 }
 
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
-                const CUtensorMap* tmOut, cudaStream_t stream) {
+                const CUtensorMap* tmOut, cudaStream_t stream, const CUtensorMap* tmOut2) {
   static bool attr_done[kMaxDevices] = {false};
   const int dev = current_device();
   if (!attr_done[dev]) {
@@ -1529,17 +1667,23 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
         for (int bn : {32, 64, 128, 192})
           if (e == cudaSuccess)
             e = cudaFuncSetAttribute(halo_kernel(cl, bn, v > 0, v > 1), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    for (int cl : {1, 2, 4})
+      for (int bn : {64, 128})
+        if (e == cudaSuccess)
+          e = cudaFuncSetAttribute(halo_kernel(cl, bn, true, true, true), cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm kernels): %s", cudaGetErrorString(e));
     cudaDeviceGetAttribute(&g_sm_counts[dev], cudaDevAttrMultiProcessorCount, dev);
     attr_done[dev] = true;
   }
   const int g_sm_count = g_sm_counts[dev];
+  // the static-scale E4M3 conv with residuals or an e4m3 ReLU copy (pf_gemm sets out2 there only with out2_e4m3)
+  const bool res8 = d.halo && d.a_e4m3 && d.a_static && (d.res1 != nullptr || d.res2 != nullptr || d.out2 != nullptr);
   {
     const long long rows = d.a_mode == 1 ? static_cast<long long>(d.NB) * d.H * d.W : d.M;
     int ktrue = 0;
     for (int s = 0; s < d.num_src; ++s) ktrue += d.k_true[s];
     const int n_true = d.ps > 1 ? d.n_logical * d.ps * d.ps : d.N;
-    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? (d.a_static ? (d.out_e4m3 ? "conv3x3_e4m3_static_q8out" : "conv3x3_e4m3_static") : "conv3x3_e4m3") : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : (d.a_e4m3 ? (d.out_e4m3 ? "linear_e4m3_q8out" : "linear_e4m3") : "linear"))),
+    note_work(2.0 * rows * ktrue * d.taps * n_true, "%s rows%lld K%dx%d N%d%s%s%s", d.taps == 9 ? (d.a_e4m3 ? (d.a_static ? (d.out_e4m3 ? "conv3x3_e4m3_static_q8out" : (res8 ? "conv3x3_e4m3_static_res" : "conv3x3_e4m3_static")) : "conv3x3_e4m3") : "conv3x3") : (d.a_mode == 1 ? "conv1x1" : (d.ps > 1 ? "convT" : (d.a_e4m3 ? (d.out_e4m3 ? "linear_e4m3_q8out" : "linear_e4m3") : "linear"))),
               rows, d.taps, ktrue, n_true, d.act ? (d.act == PF_ACT_GELU ? " gelu" : (d.act == PF_ACT_RELU ? " relu" : " softplus")) : "",
               d.gamma ? " gamma" : (d.vt ? " vt" : ""), d.w2 ? " tail" : "");
   }
@@ -1549,6 +1693,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   P.tmB = tmB;
   P.tmBh = tmBh ? *tmBh : tmB;
   P.tmOut = tmOut ? *tmOut : tmB;
+  P.tmOut2 = tmOut2 ? *tmOut2 : tmB;
   P.d = d;
   if (d.tma_out && !tmOut) return set_error("gemm: tma_out without an output tensor map");
   int ks = 0;
@@ -1561,8 +1706,9 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   int grid = P.total_tiles < g_sm_count ? P.total_tiles : g_sm_count;
   if (d.halo) {
     const bool f8 = d.a_e4m3 != 0, q8 = f8 && d.a_static != 0;
-    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n, f8, q8);
-    if (hk == nullptr) return set_error("conv3 halo: block_n %d (32, 64, 128 or 192)", d.block_n);
+    const KernelFn hk = halo_kernel(d.halo_cl, d.block_n, f8, q8, res8);
+    if (hk == nullptr)
+      return set_error("conv3 halo: block_n %d (32, 64, 128 or 192; 64 or 128 with residuals or a ReLU copy)", d.block_n);
     const int b_bytes = halo_kc(d.block_n, f8) * d.block_n * kBlockK * (f8 ? 1 : 2);     // one weight stage
     const int hstages = halo_stages(d.block_n, f8);
     size_t hsmem = 1024 + static_cast<size_t>(kHaloSlots) * halo_slot(f8) + static_cast<size_t>(hstages) * b_bytes +
@@ -1582,8 +1728,8 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       at[1].val.programmaticStreamSerializationAllowed = 1;
       cfg.attrs = at;
       cfg.numAttrs = 1;
-      static int max_clusters[kMaxDevices][3][5] = {};
-      int (&mcl)[5] = max_clusters[dev][q8 ? 2 : (f8 ? 1 : 0)];
+      static int max_clusters[kMaxDevices][4][5] = {};
+      int (&mcl)[5] = max_clusters[dev][res8 ? 3 : (q8 ? 2 : (f8 ? 1 : 0))];
       if (mcl[cl] == 0) {
         cfg.gridDim = dim3(cl * (g_sm_count / cl));
         int n = 0;
@@ -1599,7 +1745,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
       le = launch_pdl(hk, dim3(grid), dim3(kHaloThreads), hsmem, stream, P);
     }
     if (le != cudaSuccess)
-      return set_error("%s launch: %s", q8 ? "pf_conv3_halo_e4m3_q8_kernel" : (f8 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel"),
+      return set_error("%s launch: %s", res8 ? "pf_conv3_halo_e4m3_res_kernel" : (q8 ? "pf_conv3_halo_e4m3_q8_kernel" : (f8 ? "pf_conv3_halo_e4m3_kernel" : "pf_conv3_halo_kernel")),
                        cudaGetErrorString(le));
   } else {
     if (d.pp && (d.block_n % kPpBN != 0 || d.num_src != 1 || d.a_mode != 0 || !d.tma_out))
@@ -1633,7 +1779,7 @@ int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tm
   }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return set_error("pf_gemm_kernel launch: %s", cudaGetErrorString(e));
-  count_launch(d.halo ? (d.a_e4m3 ? (d.a_static ? "pf_conv3_halo_e4m3_q8_kernel" : "pf_conv3_halo_e4m3_kernel") : "pf_conv3_halo_kernel")
+  count_launch(d.halo ? (d.a_e4m3 ? (d.a_static ? (res8 ? "pf_conv3_halo_e4m3_res_kernel" : "pf_conv3_halo_e4m3_q8_kernel") : "pf_conv3_halo_e4m3_kernel") : "pf_conv3_halo_kernel")
                        : (pp8 ? "pf_gemm_pp_e4m3_kernel" : (d.pp ? "pf_gemm_pp_kernel" : "pf_gemm_kernel")));
   return 0;
 }

@@ -57,7 +57,7 @@ struct GemmDesc {
   int a_static;
   float a_scale;
   int out_e4m3;
-  float out_ratio;
+  float out_ratio;       // pf_conv3_halo_e4m3_res_kernel (bf16 output): the ratio of its e4m3 ReLU copy out2
 };
 
 int set_error(const char* fmt, ...);
@@ -110,7 +110,8 @@ constexpr int kPpBN = 128;
 // ({64, 128} and {64, 64} boxes for d.pp)
 // tmOut: output tensor map when d.tma_out != 0
 int gemm_launch(const GemmDesc& d, const CUtensorMap* tmA, const CUtensorMap& tmB, const CUtensorMap* tmBh,
-                const CUtensorMap* tmOut, cudaStream_t stream);
+                const CUtensorMap* tmOut, cudaStream_t stream,
+                const CUtensorMap* tmOut2 = nullptr);
 
 // Tensor maps (driver entry point fetched at run time; cached by key).
 int tmap_2d_bf16(CUtensorMap* out, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_cols,

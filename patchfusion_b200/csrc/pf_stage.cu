@@ -230,6 +230,64 @@ static void linear_e4m3(Ctx& c, const pf_layer& L, const void* A, long long M, i
   c.chk(pf_gemm(&d, c.stream));
 }
 
+// ---- dpt_precision 'fp8_static': the DPT decoder's 19 covered 3x3 convs (the four reassemble convs, the 14 RCU convs
+// that run, output_conv1), each with e4m3 panels and a calibrated input amax.  All or none of them run E4M3.
+static bool dpt_fp8(const pf_branch& b) {
+  const pf_layer* L[19] = {&b.rn[0], &b.rn[1], &b.rn[2], &b.rn[3], &b.ff_c1[3][1], &b.ff_c2[3][1], &b.oc1};
+  int n = 7;
+  for (int i = 0; i < 3; ++i)
+    for (int u = 0; u < 2; ++u) { L[n++] = &b.ff_c1[i][u]; L[n++] = &b.ff_c2[i][u]; }
+  for (int i = 0; i < n; ++i)
+    if (!L[i]->w8 || !L[i]->w_scale || !L[i]->a_amax || L[i]->taps != 9 || L[i]->num_src != 1) return false;
+  return true;
+}
+
+// One covered DPT conv on the e4m3 map q (one source of L.src_c[0] channels, kc bytes per pixel) at L's static scale,
+// activation `act`.  next != nullptr: the output is next's e4m3 operand map (out_ld bytes; the RCU conv1 -> conv2 hand-
+// off, pf_conv3_halo_e4m3_q8_kernel).  Otherwise a bf16 `out` plus the residuals res1 / res2 and, when copy_next is
+// given, the e4m3 ReLU copy `copy` (copy_ld bytes) at copy_next's ratio (pf_conv3_halo_e4m3_res_kernel; the q8 kernel
+// when there is neither).  Debug taps "e4m3d.<name>.in" (the e4m3 map read), ".out" (bf16, or e4m3 with next),
+// ".res1" / ".res2" (the residuals read) and ".copy" (the e4m3 ReLU copy), so a test can check each conv on exactly its
+// own inputs.
+static void conv_dpt_e4m3(Ctx& c, const char* name, const pf_layer& L, const void* q, int kc, int T, int H, int W, int act,
+                          void* out, int out_ld, const pf_layer* next, const Map* res1, const Map* res2, void* copy,
+                          int copy_ld, const pf_layer* copy_next) {
+  if (!c.live()) return;
+  pf_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.num_src = 1; d.a_mode = 1;
+  d.a_ptr[0] = q;
+  d.a_c[0] = pad_to(L.src_c[0], 8); d.a_ld[0] = kc;
+  d.NB = T; d.H = H; d.W = W;
+  GemmOpt o; o.act = act; o.res1 = res1; o.res2 = res2;
+  gemm_desc_common(d, L, o, out, 0, out_ld);
+  d.w_ptr = L.w8;
+  d.a_e4m3 = 1; d.s_w = L.w_scale;
+  d.a_static = 1; d.a_scale = static_scale(*L.a_amax);
+  if (next != nullptr) { d.out_e4m3 = 1; d.out_ratio = static_ratio(*next->a_amax); }
+  if (copy_next != nullptr) { d.out2 = copy; d.out2_ld = copy_ld; d.out2_e4m3 = 1; d.out2_ratio = static_ratio(*copy_next->a_amax); }
+  c.chk(pf_gemm(&d, c.stream));
+  if (c.tap != nullptr && c.live()) {
+    char nm[64];
+    const long long rows = static_cast<long long>(T) * H * W;
+    snprintf(nm, sizeof(nm), "e4m3d.%s.in", name);
+    c.tap_out(nm, q, 2, rows, kc, kc);
+    snprintf(nm, sizeof(nm), "e4m3d.%s.out", name);
+    if (next != nullptr) c.tap_out(nm, out, 2, rows, out_ld, out_ld);
+    else c.tap_out(nm, out, 0, rows, L.N, out_ld);
+    const Map* rs[2] = {res1, res2};
+    for (int i = 0; i < 2; ++i)
+      if (rs[i] != nullptr) {
+        snprintf(nm, sizeof(nm), "e4m3d.%s.res%d", name, i + 1);
+        c.tap_out(nm, rs[i]->p, 0, rows, rs[i]->C, rs[i]->ld);
+      }
+    if (copy_next != nullptr) {
+      snprintf(nm, sizeof(nm), "e4m3d.%s.copy", name);
+      c.tap_out(nm, copy, 2, rows, copy_ld, copy_ld);
+    }
+  }
+}
+
 // 3x3 / 1x1 conv over up to three channel-concatenated NHWC sources
 static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_f32, int out_ld,
                       const GemmOpt& o = GemmOpt()) {
@@ -590,33 +648,100 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
       lay[i] = o;
     }
   }
+  // dpt_precision 'fp8_static' (dpt_fp8): layer{i}_rn reads lay[i] through one static quantize and writes the bf16
+  // rn[i] and the e4m3 ReLU copy of it that the first RCU conv1 reading it takes; an RCU conv1 reads that copy and
+  // writes its conv2's e4m3 operand; conv2 adds x (and the path) and writes bf16 y, plus the e4m3 ReLU copy the next
+  // unit's conv1 reads; output_conv1 reads the resized p1 through one static quantize.  No bf16 ReLU copy or t map of
+  // a covered conv exists.  The bf16 path keeps the calibration taps "amaxd.<conv>" on each covered conv's bf16 input.
+  const bool f8 = dpt_fp8(Wb);
+  static const char* const kRn[4] = {"layer1_rn", "layer2_rn", "layer3_rn", "layer4_rn"};
+  char dn[48];
+  auto amax_tap = [&](const char* conv, const Map& m) {
+    if (c.tap == nullptr) return;
+    char an[64];
+    snprintf(an, sizeof(an), "amaxd.%s", conv);
+    c.tap_out(an, m.p, 0, m.rows(), m.C, m.ld);
+  };
+  // the conv1 that reads rn[i]'s ReLU: refinenet4's only unit for rn[3], the first unit of refinenet{i+1} otherwise
+  auto rn_reader = [&](int i) -> const pf_layer& { return i == 3 ? Wb.ff_c1[3][1] : Wb.ff_c1[i][0]; };
   Map rn[4], rn_relu[4];
+  uint8_t* rn8[4] = {nullptr, nullptr, nullptr, nullptr};
   for (int i = 0; i < 4; ++i) {
-    rn_relu[i] = c.map(lay[i].B, lay[i].H, lay[i].W, C);
-    GemmOpt g; g.relu_copy = &rn_relu[i];
-    rn[i] = conv1(c, Wb.rn[i], lay[i], g);
+    if (f8) {
+      int kc = 0;
+      const Map* a[1] = {&lay[i]};
+      void* q = quant_static(c, Wb.rn[i], a, 1, &kc);
+      rn[i] = c.map(lay[i].B, lay[i].H, lay[i].W, C);
+      rn8[i] = static_cast<uint8_t*>(c.alloc(static_cast<size_t>(rn[i].rows()) * pad_to(C, 64)));
+      conv_dpt_e4m3(c, kRn[i], Wb.rn[i], q, kc, lay[i].B, lay[i].H, lay[i].W, PF_ACT_NONE, rn[i].p, rn[i].ld, nullptr,
+                    nullptr, nullptr, rn8[i], pad_to(C, 64), &rn_reader(i));
+    } else {
+      amax_tap(kRn[i], lay[i]);
+      rn_relu[i] = c.map(lay[i].B, lay[i].H, lay[i].W, C);
+      GemmOpt g; g.relu_copy = &rn_relu[i];
+      rn[i] = conv1(c, Wb.rn[i], lay[i], g);
+    }
   }
   // ResidualConvUnit: y = conv2(relu(conv1(relu(x)))) + x (+ extra); optionally also relu(y)
   auto rcu = [&](int wi, int u, const Map& xin, const Map& xrelu, const Map* extra, Map* relu_copy) -> Map {
+    char n1[48], n2[48];
+    snprintf(n1, sizeof(n1), "refinenet%d.resConfUnit%d.conv1", wi, u);
+    snprintf(n2, sizeof(n2), "refinenet%d.resConfUnit%d.conv2", wi, u);
+    amax_tap(n1, xrelu);
     GemmOpt g1; g1.act = PF_ACT_RELU;
     Map t = conv1(c, Wb.ff_c1[wi - 1][u - 1], xrelu, g1);
+    amax_tap(n2, t);
     GemmOpt g2; g2.res1 = &xin; g2.res2 = extra;
     if (relu_copy) { *relu_copy = c.map(xin.B, xin.H, xin.W, C); g2.relu_copy = relu_copy; }
     return conv1(c, Wb.ff_c2[wi - 1][u - 1], t, g2);
   };
+  // the same unit in FP8: x8 is the e4m3 ReLU copy of xin at conv1's ratio; copy8 (when given) receives y's e4m3 ReLU
+  // copy at the ratio of the next unit's conv1
+  auto rcu8 = [&](int wi, int u, const Map& xin, const uint8_t* x8, const Map* extra, uint8_t** copy8) -> Map {
+    const pf_layer& c1 = Wb.ff_c1[wi - 1][u - 1];
+    const pf_layer& c2 = Wb.ff_c2[wi - 1][u - 1];
+    const int kc = pad_to(C, 64);
+    uint8_t* t8 = static_cast<uint8_t*>(c.alloc(static_cast<size_t>(xin.rows()) * kc));
+    snprintf(dn, sizeof(dn), "refinenet%d.resConfUnit%d.conv1", wi, u);
+    conv_dpt_e4m3(c, dn, c1, x8, kc, xin.B, xin.H, xin.W, PF_ACT_RELU, t8, kc, &c2, nullptr, nullptr, nullptr, 0, nullptr);
+    Map y = c.map(xin.B, xin.H, xin.W, C);
+    if (copy8 != nullptr) *copy8 = static_cast<uint8_t*>(c.alloc(static_cast<size_t>(xin.rows()) * kc));
+    snprintf(dn, sizeof(dn), "refinenet%d.resConfUnit%d.conv2", wi, u);
+    conv_dpt_e4m3(c, dn, c2, t8, kc, xin.B, xin.H, xin.W, PF_ACT_NONE, y.p, y.ld, nullptr, &xin, extra,
+                  copy8 != nullptr ? *copy8 : nullptr, kc, copy8 != nullptr ? &Wb.ff_c1[wi - 1][1] : nullptr);
+    return y;
+  };
   // FeatureFusionBlock; the 1x1 out_conv commutes with the bilinear upsample and runs at the low resolution
-  auto ffb = [&](int wi, const Map* path, const Map& skip, const Map& skip_relu, int OH, int OW) -> Map {
-    Map s = skip, s_relu = skip_relu;
-    if (path != nullptr) s = rcu(wi, 1, skip, skip_relu, path, &s_relu);
-    Map y = rcu(wi, 2, s, s_relu, nullptr, nullptr);
+  auto ffb = [&](int wi, const Map* path, int i, int OH, int OW) -> Map {
+    Map s = rn[i], y;
+    if (f8) {
+      uint8_t* s8 = rn8[i];
+      if (path != nullptr) s = rcu8(wi, 1, rn[i], rn8[i], path, &s8);
+      y = rcu8(wi, 2, s, s8, nullptr, nullptr);
+    } else {
+      Map s_relu = rn_relu[i];
+      if (path != nullptr) s = rcu(wi, 1, rn[i], rn_relu[i], path, &s_relu);
+      y = rcu(wi, 2, s, s_relu, nullptr, nullptr);
+    }
     y = conv1(c, Wb.ff_out[wi - 1], y);
     return resize(c, y, OH, OW);
   };
-  Map p4 = ffb(4, nullptr, rn[3], rn_relu[3], rn[2].H, rn[2].W);
-  Map p3 = ffb(3, &p4, rn[2], rn_relu[2], rn[1].H, rn[1].W);
-  Map p2 = ffb(2, &p3, rn[1], rn_relu[1], rn[0].H, rn[0].W);
-  Map p1 = ffb(1, &p2, rn[0], rn_relu[0], rn[0].H * 2, rn[0].W * 2);
-  Map o = conv1(c, Wb.oc1, p1);
+  Map p4 = ffb(4, nullptr, 3, rn[2].H, rn[2].W);
+  Map p3 = ffb(3, &p4, 2, rn[1].H, rn[1].W);
+  Map p2 = ffb(2, &p3, 1, rn[0].H, rn[0].W);
+  Map p1 = ffb(1, &p2, 0, rn[0].H * 2, rn[0].W * 2);
+  Map o;
+  if (f8) {
+    int kc = 0;
+    const Map* a[1] = {&p1};
+    void* q = quant_static(c, Wb.oc1, a, 1, &kc);
+    o = c.map(p1.B, p1.H, p1.W, Wb.oc1.N);
+    conv_dpt_e4m3(c, "output_conv1", Wb.oc1, q, kc, p1.B, p1.H, p1.W, PF_ACT_NONE, o.p, o.ld, nullptr, nullptr, nullptr,
+                  nullptr, 0, nullptr);
+  } else {
+    amax_tap("output_conv1", p1);
+    o = conv1(c, Wb.oc1, p1);
+  }
   o = resize(c, o, H, W);
   MapF rel = c.mapf(B, H, W, 1, 8);
   if (c.live()) {     // only column 0 is produced (fused 32 -> 1 layer); the 7 pad columns feed zero weights and must be finite

@@ -24,7 +24,8 @@ import torch.nn.functional as F
 from . import lib, ops
 from .ops import ACT_GELU, ACT_NONE, ACT_RELU, ACT_SOFTPLUS, call, pad_to, stream_ptr
 from .params import FP8_LAYERS, VIT_FP8_LINEARS, WINDOW, branch_hparams, fusion_fp8_amax, fusion_precision, \
-    guided_fusion_hparams, normed_attractors, vit_fp8_amax, vit_fp8_layers, vit_precision, _get
+    guided_fusion_hparams, normed_attractors, vit_fp8_amax, vit_fp8_layers, vit_precision, DPT_FP8_CONVS, dpt_fp8_amax, \
+    dpt_fp8_layers, dpt_precision, _get
 
 BF16, F32 = torch.bfloat16, torch.float32
 
@@ -71,15 +72,22 @@ class Engine:
         # vit_precision 'fp8_static': qkv, fc1 and fc2 of both encoders get e4m3 panels next to their bf16 ones
         # (calibration runs the bf16 encoder).  c_branch carries the calibrated input amax (set_vit_fp8_amax), c_branch_bf16
         # is the same stage without them.
+        # dpt_precision 'fp8_static' does the same for the 19 DPT_FP8_CONVS of each decoder (set_dpt_fp8_amax); their
+        # e4m3 panels are left out of c_branch_bf16, which runs them in bf16.
         self.vit_fp8_static = vit_precision(config) == 'fp8_static'
+        self.dpt_fp8_static = dpt_precision(config) == 'fp8_static'
         self.W = {}
         self._pack_all()
         self.sd = None   # fp32 originals are no longer needed on the device
         self.c_branch = {b: self._c_branch(b) for b in ('coarse', 'fine') if b in self.parts}
         self.c_branch_bf16 = dict(self.c_branch)
         self.vit_amax = None
+        self.dpt_amax = None
+        self._branch_amax = {}
         if self.vit_fp8_static:
             self.set_vit_fp8_amax(vit_fp8_amax(config))
+        if self.dpt_fp8_static:
+            self.set_dpt_fp8_amax(dpt_fp8_amax(config))
         self.c_fusion = self._c_fusion() if 'fusion' in self.parts else None
         # 'fp8_static': c_fusion carries the calibrated input amax of each FP8 conv (set_fp8_amax); c_fusion_tiles is the
         # same stage with per-tile scales, which calibration runs.  `calib` (a dict while PatchFusion.calibrate_fp8 runs)
@@ -106,6 +114,10 @@ class Engine:
     # ------------------------------------------------------------------ weight packing
     def _w(self, k):
         return self.sd[k]
+
+    def _dpt_conv(self, name, bias=True):
+        """a DPT conv of DPT_FP8_CONVS: its e4m3 panel too under dpt_precision 'fp8_static'"""
+        return self._conv(name, bias=bias, fp8='keep_bf16' if self.dpt_fp8_static else None)
 
     def _conv(self, name, src_c=None, bias=True, fp8=None):
         """fp8: None packs bf16; 'only' / 'keep_bf16' packs e4m3 (pack_weight_e4m3), the latter with the bf16 panel
@@ -196,14 +208,16 @@ class Engine:
         rs3.taps, rs3.src_c = 1, [9 * oc[3]]          # consumed as a plain GEMM over pf_im2col_3x3_s2 rows
         Wd['rs3'] = rs3
         for i in range(4):
-            Wd['rn%d' % i] = self._conv(dh + 'scratch.layer%d_rn' % (i + 1), bias=False)
+            Wd['rn%d' % i] = self._dpt_conv(dh + 'scratch.layer%d_rn' % (i + 1), bias=False)
         for i in range(1, 5):
             r = dh + 'scratch.refinenet%d.' % i
             Wd['ff%d.out' % i] = self._conv(r + 'out_conv')
             for u in (1, 2):
-                Wd['ff%d.u%d.c1' % (i, u)] = self._conv(r + 'resConfUnit%d.conv1' % u)
-                Wd['ff%d.u%d.c2' % (i, u)] = self._conv(r + 'resConfUnit%d.conv2' % u)
-        Wd['oc1'] = self._conv(dh + 'scratch.output_conv1')
+                # refinenet4's resConfUnit1 never runs (its FeatureFusionBlock has no second input): bf16 only
+                conv = self._conv if (i, u) == (4, 1) else self._dpt_conv
+                Wd['ff%d.u%d.c1' % (i, u)] = conv(r + 'resConfUnit%d.conv1' % u)
+                Wd['ff%d.u%d.c2' % (i, u)] = conv(r + 'resConfUnit%d.conv2' % u)
+        Wd['oc1'] = self._dpt_conv(dh + 'scratch.output_conv1')
         Wd['oc2.0'] = self._conv(dh + 'scratch.output_conv2.0')
         Wd['oc2.tail'] = (self._w(dh + 'scratch.output_conv2.2.weight').reshape(1, -1).float().contiguous(),
                           self._f32(dh + 'scratch.output_conv2.2.bias'))
@@ -292,8 +306,10 @@ class Engine:
         H.min_depth, H.max_depth = float(_get(depth_cfg, 'min_depth', 1e-3)), float(_get(depth_cfg, 'max_depth', 10))
         return H
 
-    def _c_branch(self, which, amax=None):
-        """amax: {'<i>.<qkv|fc1|fc2>': address of its fp32 input amax} of a calibrated 'fp8_static' encoder, or None"""
+    def _c_branch(self, which, amax=None, dpt_amax=None):
+        """amax: {'<i>.<qkv|fc1|fc2>': address of its fp32 input amax} of a calibrated 'fp8_static' encoder, or None;
+        dpt_amax: {conv of DPT_FP8_CONVS: address of its fp32 input amax} of a calibrated 'fp8_static' decoder, or None
+        (the decoder then runs in bf16: its e4m3 panels are not passed)"""
         from . import stage
         Wd, hp = self.W[which], self.hp[which]
         B = stage.PfBranch()
@@ -325,6 +341,18 @@ class Engine:
                 B.ff_c2[i][u - 1] = stage.layer(Wd['ff%d.u%d.c2' % (i + 1, u)])
         B.rs0, B.rs1, B.rs3 = stage.layer(Wd['rs0']), stage.layer(Wd['rs1']), stage.layer(Wd['rs3'])
         B.oc1 = stage.layer(Wd['oc1'])
+        dpt = [B.rn[i] for i in range(4)] + [B.ff_c1[i][u] for i in range(3) for u in (0, 1)] + \
+            [B.ff_c2[i][u] for i in range(3) for u in (0, 1)] + [B.ff_c1[3][1], B.ff_c2[3][1], B.oc1]
+        names = ['layer%d_rn' % i for i in range(1, 5)] + \
+            ['refinenet%d.resConfUnit%d.conv1' % (i, u) for i in (1, 2, 3) for u in (1, 2)] + \
+            ['refinenet%d.resConfUnit%d.conv2' % (i, u) for i in (1, 2, 3) for u in (1, 2)] + \
+            ['refinenet4.resConfUnit2.conv1', 'refinenet4.resConfUnit2.conv2', 'output_conv1']
+        assert sorted(names) == sorted(DPT_FP8_CONVS)
+        for L, n in zip(dpt, names):
+            if dpt_amax is None:
+                L.w8, L.w_scale = None, None
+            else:
+                L.a_amax = dpt_amax[n]
         B.oc2 = stage.layer(Wd['oc2.0'], Wd['oc2.tail'])
         B.conv2 = stage.layer(Wd['conv2'])
         B.head = self._c_head(Wd['head'], hp, self.bcfg[which], True, self.bcfg[which])
@@ -350,20 +378,38 @@ class Engine:
         if table is None:
             self.vit_amax, self.c_branch = None, dict(self.c_branch_bf16)
             return
-        table = dict(table)
-        names = vit_fp8_layers(self.cfg)
-        arr = (ct.c_float * len(names))(*[table[k] for k in names])
-        self._keep.append(arr)
-        addr = {k: ct.addressof(arr) + 4 * i for i, k in enumerate(names)}
-        self.c_branch = {b: self._c_branch(b, {k[len(b) + 1:]: a for k, a in addr.items() if k.startswith(b + '.')})
-                         for b in self.c_branch_bf16}
-        self.vit_amax = table
+        self.vit_amax = dict(table)
+        self._set_branch_amax(vit_fp8_layers(self.cfg), self.vit_amax, 'vit')
+
+    def set_dpt_fp8_amax(self, table):
+        """dpt_precision 'fp8_static': the calibrated input amax of the decoders' DPT_FP8_CONVS ({name of
+        dpt_fp8_layers: float}, validated), or None (no table: the branches refuse to run, calibration still can).  Read
+        when a stage is issued, so graphs captured before a change must be dropped (PatchFusion.engine does)."""
+        self.dpt_amax = dict(table) if table is not None else None
+        self._set_branch_amax(dpt_fp8_layers(self.cfg), self.dpt_amax, 'dpt')
+
+    def _set_branch_amax(self, names, table, kind):
+        """re-points c_branch at the current ViT and DPT tables (kind: which of them `table` is)"""
+        if table is None:
+            self._branch_amax.pop(kind, None)
+        else:
+            arr = (ct.c_float * len(names))(*[table[k] for k in names])
+            self._keep.append(arr)
+            self._branch_amax[kind] = {k: ct.addressof(arr) + 4 * i for i, k in enumerate(names)}
+
+        def per_branch(kind, b):
+            addr = self._branch_amax.get(kind)
+            return None if addr is None else {k[len(b) + 1:]: a for k, a in addr.items() if k.startswith(b + '.')}
+        self.c_branch = {b: self._c_branch(b, per_branch('vit', b), per_branch('dpt', b)) for b in self.c_branch_bf16}
 
     def _branch_struct(self, which):
         if self.calib is not None:
             return self.c_branch_bf16[which]
         if self.vit_fp8_static and self.vit_amax is None:
             raise RuntimeError("vit_precision 'fp8_static' needs the calibrated input scales `vit_fp8_amax`: run "
+                               "PatchFusion.calibrate_fp8 (or tools/calibrate_fp8.py) first")
+        if self.dpt_fp8_static and self.dpt_amax is None:
+            raise RuntimeError("dpt_precision 'fp8_static' needs the calibrated input scales `dpt_fp8_amax`: run "
                                "PatchFusion.calibrate_fp8 (or tools/calibrate_fp8.py) first")
         return self.c_branch[which]
 
@@ -436,8 +482,8 @@ class Engine:
     def _tap_cb(self, arena, taps):
         def cb(user, name, ptr, is_f32, rows, cols, ld):
             # is_f32: 0 bf16, 1 fp32, 2 e4m3 bytes (the static FP8 convs' operand maps)
-            if name.startswith(b'amaxv.'):
-                return      # the bf16 encoder's calibration inputs (_calib_vit_cb): not kept
+            if name.startswith(b'amaxv.') or name.startswith(b'amaxd.'):
+                return      # the bf16 branch's calibration inputs (_calib_vit_cb): not kept
             t = self._view(arena, ptr, (rows, ld), (BF16, F32, torch.uint8)[is_f32])
             taps[name.decode()] = t[:, :cols].clone()
         return cb
@@ -455,12 +501,15 @@ class Engine:
         return cb
 
     def _calib_vit_cb(self, arena, which):
-        """calibration of the 'fp8_static' encoders: fold the amax of each E4M3 linear's bf16 input (tap
-        "amaxv.<i>.<lin>" of the bf16 stage) into calib['<which>.<i>.<lin>'], NaN-propagating, on the stream the branch
-        is issued on (the current stream, as the launches)"""
+        """calibration of the 'fp8_static' encoders and decoders: fold the amax of each E4M3 linear's / DPT conv's bf16
+        input (tap "amaxv.<i>.<lin>" / "amaxd.<conv>" of the bf16 stage) into calib['<which>.<i>.<lin>'] /
+        calib['<which>.<conv>'], NaN-propagating, on the stream the branch is issued on (the current stream, as the
+        launches)"""
+        prefixes = tuple(p for p, on in (('amaxv.', self.vit_fp8_static), ('amaxd.', self.dpt_fp8_static)) if on)
+
         def cb(user, name, ptr, is_f32, rows, cols, ld):
             name = name.decode()
-            if not name.startswith('amaxv.'):
+            if not name.startswith(prefixes):
                 return
             lo, hi = torch.aminmax(self._view(arena, ptr, (rows, ld), BF16)[:, :cols])
             m = torch.maximum(-lo, hi).float()
@@ -483,7 +532,7 @@ class Engine:
             arena, off = ws
         assert images.dtype == F32 and images.is_contiguous() and off % 256 == 0 and off + need <= arena.numel()
         tap = self._tap_cb(arena, taps) if taps is not None else None
-        if tap is None and self.calib is not None and self.vit_fp8_static:
+        if tap is None and self.calib is not None and (self.vit_fp8_static or self.dpt_fp8_static):
             tap = self._calib_vit_cb(arena, which)
         out = stage.branch_forward(cb, images, B, arena.data_ptr() + off, need, tap)
         H, W = self.P

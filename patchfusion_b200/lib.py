@@ -45,6 +45,7 @@ class GemmDesc(C.Structure):
         ('rs_h', C.c_int32 * 3), ('rs_w', C.c_int32 * 3),
         ('a_e4m3', C.c_int32), ('s_a', C.c_void_p), ('s_w', C.c_void_p),
         ('a_static', C.c_int32), ('a_scale', C.c_float), ('out_e4m3', C.c_int32), ('out_ratio', C.c_float),
+        ('out2_e4m3', C.c_int32), ('out2_ratio', C.c_float),
     ]
 
 

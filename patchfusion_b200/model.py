@@ -14,7 +14,7 @@ import torch
 import torch.nn as nn
 
 from .params import FP8_LAYERS, ParamTree, _get, fusion_fp8_amax, fusion_precision, state_layout, synthetic_state_dict, relative_position_index, \
-    vit_fp8_amax, vit_fp8_layers, vit_precision
+    vit_fp8_amax, vit_fp8_layers, vit_precision, dpt_fp8_amax, dpt_fp8_layers, dpt_precision
 
 try:
     from huggingface_hub import PyTorchModelHubMixin
@@ -515,6 +515,8 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
         self.resizer = Resize(config.patch_process_shape[1], config.patch_process_shape[0])
         self.vit_precision = vit_precision(config)           # ValueError on anything but 'bf16' / 'fp8_static'
         vit_fp8_amax(config)                                 # ValueError on a malformed ViT calibration table
+        self.dpt_precision = dpt_precision(config)           # ValueError on anything but 'bf16' / 'fp8_static'
+        dpt_fp8_amax(config)                                 # ValueError on a malformed DPT calibration table
         self._build_tree(state_layout(config))      # raises ValueError / NotImplementedError like the reference
         self.consistency_training = False
         self._runtime_init()
@@ -573,23 +575,30 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
                 if table != self._engine.vit_amax:
                     self._engine.set_vit_fp8_amax(table)
                     self._graphs = {}
+            if self._engine.dpt_fp8_static:
+                table = dpt_fp8_amax(self.config)
+                if table != self._engine.dpt_amax:
+                    self._engine.set_dpt_fp8_amax(table)
+                    self._graphs = {}
         return self._engine
 
     @torch.no_grad()
     def calibrate_fp8(self, image_lr, image_hr, cai_mode='m1', process_num=4, tile_cfg=None, reset=False):
-        """Post-training calibration of the static FP8 U-Net ('fp8' and 'fp8_static' models) and of the 'fp8_static'
-        ViT encoders: runs forward(mode='infer') on the given images (the same arguments: batches, mixed geometry, rN
-        modes drawing from `random`) with the per-tile 'fp8' U-Net arithmetic and the bf16 encoders on this model's
-        panels, and takes, for each of the 34 FP8 convs and each E4M3 ViT linear, the maximum over all tiles and images
-        of its input's amax.  Each table is merged by max into config['fusion_fp8_amax'] / config['vit_fp8_amax']
-        (reset=True starts from empty tables), which 'fp8_static' then runs with.  Returns the U-Net table, or the ViT
-        table when the U-Net is not FP8.  Runs eagerly: no graph of it is kept, and the graphs of earlier forwards are
-        dropped."""
+        """Post-training calibration of the static FP8 U-Net ('fp8' and 'fp8_static' models), of the 'fp8_static'
+        ViT encoders and of the 'fp8_static' DPT decoders: runs forward(mode='infer') on the given images (the same
+        arguments: batches, mixed geometry, rN modes drawing from `random`) with the per-tile 'fp8' U-Net arithmetic and
+        the bf16 branches on this model's panels, and takes, for each of the 34 FP8 convs, each E4M3 ViT linear and each
+        E4M3 DPT conv, the maximum over all tiles and images of its input's amax.  Each table is merged by max into
+        config['fusion_fp8_amax'] / config['vit_fp8_amax'] / config['dpt_fp8_amax'] (reset=True starts from empty
+        tables), which 'fp8_static' then runs with.  Returns the U-Net table, else the ViT table, else the DPT table.
+        Runs eagerly: no graph of it is kept, and the graphs of earlier forwards are dropped."""
         unet = self.fusion_precision in ('fp8', 'fp8_static')
         vit = self.vit_precision == 'fp8_static'
-        if not unet and not vit:
-            raise ValueError("calibrate_fp8 needs fusion_precision 'fp8' or 'fp8_static', or vit_precision 'fp8_static' "
-                             "(this model: %r, %r)" % (self.fusion_precision, self.vit_precision))
+        dpt = self.dpt_precision == 'fp8_static'
+        if not unet and not vit and not dpt:
+            raise ValueError("calibrate_fp8 needs fusion_precision 'fp8' or 'fp8_static', vit_precision 'fp8_static' or "
+                             "dpt_precision 'fp8_static' (this model: %r, %r, %r)"
+                             % (self.fusion_precision, self.vit_precision, self.dpt_precision))
         eng = self.engine()
         eng.calib = {}
         graphs, self.use_cuda_graphs = self.use_cuda_graphs, False
@@ -602,7 +611,8 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             self._graphs = {}
         hub = getattr(self, '_hub_mixin_config', None)
         for on, key, names, check in ((unet, 'fusion_fp8_amax', FP8_LAYERS, fusion_fp8_amax),
-                                      (vit, 'vit_fp8_amax', vit_fp8_layers(self.config), vit_fp8_amax)):
+                                      (vit, 'vit_fp8_amax', vit_fp8_layers(self.config), vit_fp8_amax),
+                                      (dpt, 'dpt_fp8_amax', dpt_fp8_layers(self.config), dpt_fp8_amax)):
             if not on:
                 continue
             missing = [k for k in names if k not in found]
@@ -617,7 +627,7 @@ class PatchFusion(TiledModel, PyTorchModelHubMixin):
             if isinstance(hub, dict):               # the config save_pretrained writes
                 hub[key] = dict(self.config[key])
         self.engine()
-        return dict(self.config['fusion_fp8_amax'] if unet else self.config['vit_fp8_amax'])
+        return dict(self.config['fusion_fp8_amax' if unet else ('vit_fp8_amax' if vit else 'dpt_fp8_amax')])
 
     def invalidate(self):
         super().invalidate()

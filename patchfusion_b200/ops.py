@@ -161,10 +161,13 @@ def quantize_e4m3_static(srcs, amax, src_c=None, out=None):
     return out
 
 
-def conv3_e4m3_static(pw, q, amax, out, next_amax=None, act=ACT_RELU, block_n=0):
+def conv3_e4m3_static(pw, q, amax, out, next_amax=None, act=ACT_RELU, block_n=0, res1=None, res2=None, copy=None,
+                      copy_amax=None):
     """The static-scale E4M3 halo conv (pf_conv3_halo_e4m3_q8_kernel): q from quantize_e4m3_static at `amax`, pw from
     pack_weight_e4m3.  next_amax None: out bf16 NHWC [T,H,W,ld]; else out is the uint8 e4m3 map [T,H,W,ld >= pad64(N)]
-    written at next_amax's ratio (the next conv's operand)."""
+    written at next_amax's ratio (the next conv's operand).
+    res1 / res2 (bf16 NHWC [T,H,W,ld], added after the bias) and copy (the uint8 e4m3 map [T,H,W,ld >= pad64(N)] that
+    receives the bf16 output's ReLU at copy_amax's ratio) run pf_conv3_halo_e4m3_res_kernel, with a bf16 out."""
     T, H, W, kc = q.shape
     assert q.dtype == torch.uint8 and kc == sum(pad_to(c, 64) for c in pw.src_c) and pw.taps == 9
     d = GemmDesc()
@@ -185,6 +188,15 @@ def conv3_e4m3_static(pw, q, amax, out, next_amax=None, act=ACT_RELU, block_n=0)
     d.a_static, d.a_scale = 1, e4m3_static_scale(amax)
     if next_amax is not None:
         d.out_e4m3, d.out_ratio = 1, e4m3_static_ratio(next_amax)
+    for i, r in enumerate((res1, res2)):
+        if r is not None:
+            assert r.dtype == torch.bfloat16 and r.is_contiguous() and tuple(r.shape[:3]) == (T, H, W)
+            setattr(d, 'res%d' % (i + 1), r.data_ptr())
+            d.res_ld = r.shape[-1]
+    if copy is not None:
+        assert copy.dtype == torch.uint8 and copy.is_contiguous() and tuple(copy.shape[:3]) == (T, H, W)
+        d.out2, d.out2_ld = copy.data_ptr(), copy.shape[-1]
+        d.out2_e4m3, d.out2_ratio = 1, e4m3_static_ratio(copy_amax)
     call('pf_gemm', C.byref(d), stream_ptr())
     return d
 

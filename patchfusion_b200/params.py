@@ -125,6 +125,53 @@ def vit_fp8_amax(config):
     return out
 
 
+DPT_PRECISIONS = ('bf16', 'fp8_static')
+# The DPT decoder's 3x3 convs that run E4M3 under dpt_precision 'fp8_static', by their names in each branch's
+# depth_head.scratch: the four reassemble convs, the ResidualConvUnits that run (refinenet4 uses only resConfUnit2)
+# and output_conv1
+DPT_FP8_CONVS = tuple(['layer%d_rn' % i for i in range(1, 5)] +
+                      ['refinenet%d.resConfUnit%d.conv%d' % (i, u, k) for i in (1, 2, 3) for u in (1, 2) for k in (1, 2)] +
+                      ['refinenet4.resConfUnit2.conv%d' % k for k in (1, 2)] + ['output_conv1'])
+
+
+def dpt_precision(config):
+    """Top-level `dpt_precision`: what the DPT decoders' covered 3x3 convs (DPT_FP8_CONVS) of both branches compute in.
+    'bf16' (default), or 'fp8_static': E4M3 operands with one calibrated scale per conv input (`dpt_fp8_amax`,
+    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision and vit_precision."""
+    p = _get(config, 'dpt_precision', 'bf16')
+    if p not in DPT_PRECISIONS:
+        raise ValueError("dpt_precision should be one of 'bf16', 'fp8_static'")
+    return p
+
+
+def dpt_fp8_layers(config=None):
+    """The names of dpt_fp8_amax: '{coarse|fine}.<conv>' for every conv of DPT_FP8_CONVS, 38 in all"""
+    return tuple('%s.%s' % (b, n) for b in ('coarse', 'fine') for n in DPT_FP8_CONVS)
+
+
+def dpt_fp8_amax(config):
+    """Top-level `dpt_fp8_amax`: the calibrated amax of each E4M3 DPT conv's input, {name of dpt_fp8_layers: float >= 0}
+    with exactly those 38 names, or None when the config has no table.  Anything else raises ValueError."""
+    t = _get(config, 'dpt_fp8_amax', None)
+    if t is None:
+        return None
+    names = dpt_fp8_layers(config)
+    if not isinstance(t, dict):
+        raise ValueError('dpt_fp8_amax should be a dict of the %d DPT conv names to their input amax' % len(names))
+    known = set(names)
+    missing = [k for k in names if k not in t]
+    unknown = sorted(str(k) for k in t if k not in known)
+    if missing or unknown:
+        raise ValueError('dpt_fp8_amax: missing layers %s, unknown layers %s' % (missing, unknown))
+    out = {}
+    for k in names:
+        v = t[k]
+        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
+            raise ValueError('dpt_fp8_amax[%r] = %r: a finite float >= 0 is required' % (k, v))
+        out[k] = float(v)
+    return out
+
+
 def branch_hparams(branch_cfg):
     enc = _get(branch_cfg, 'midas_model_type')
     if enc not in ENCODERS:

@@ -7,6 +7,8 @@ Builds the model as tools/test.py does (same config, checkpoint, dataset and til
 'fp8_static', runs PatchFusion.calibrate_fp8 over the first N images of the dataset (read and ingested as the
 evaluation reads them) and writes a save_pretrained directory whose config carries fusion_precision 'fp8_static' and the
 calibration table `fusion_fp8_amax`.  `tools/test.py <config.py> --ckp-path DIR` then evaluates the calibrated model.
+A config that selects dpt_precision 'fp8_static' (`--cfg-options model.config.dpt_precision=fp8_static`) gets the DPT
+decoders' table `dpt_fp8_amax` filled, written and printed too.
 """
 import argparse
 import json
@@ -49,6 +51,9 @@ def main(argv=None):
     # the same weights in an 'fp8_static' model (the table starts empty: calibrate_fp8 fills it)
     conf = dict(src.config.to_dict(), fusion_precision='fp8_static')
     conf.pop('fusion_fp8_amax', None)
+    dpt = conf.get('dpt_precision', 'bf16') == 'fp8_static'     # the DPT decoders' table too
+    if dpt:
+        conf.pop('dpt_fp8_amax', None)
     model = PatchFusion(conf)
     model.load_state_dict(src.state_dict(), strict=True)
     del src
@@ -65,7 +70,10 @@ def main(argv=None):
     if table is None:
         raise SystemExit('calibrate_fp8: the dataset has no images')
     model.save_pretrained(args.out)
-    print(json.dumps(dict(images=n, fusion_fp8_amax=table), indent=1))
+    out = dict(images=n, fusion_fp8_amax=table)
+    if dpt:
+        out['dpt_fp8_amax'] = dict(model.config['dpt_fp8_amax'])
+    print(json.dumps(out, indent=1))
     return table
 
 
