@@ -147,6 +147,187 @@ def test_crop_resize_and_unet_input(cuda):
     assert (u[..., 5:] == 0).all()
 
 
+# ---------------------------------------------------------------------------------------------------- as the stages call
+# The argument forms of csrc/pf_stage.cu: channel count pad8(C), row pitches wider than that.  The source columns
+# [pad8(C), ld) and the images past the batch hold NaN (pf_maxpool2: 1e30, which fmaxf cannot drop), the outputs a
+# sentinel; every value is compared with an fp64 reference on the bf16-rounded inputs.
+SENTINEL = -77.0
+
+
+def _poisoned_nhwc(x, C, ld, extra=1, fill=float('nan')):
+    """fp32 [B, H, W, C] -> bf16 [B + extra, H, W, ld]: channels [C, pad8(C)) zero (as every producer writes them),
+    [pad8(C), ld) and the `extra` images past the batch `fill`"""
+    from patchfusion_b200 import ops
+    B = x.shape[0]
+    out = torch.full((B + extra,) + tuple(x.shape[1:3]) + (ld,), fill, dtype=torch.bfloat16, device=x.device)
+    out[:B, ..., :ops.pad_to(C, 8)] = 0
+    out[:B, ..., :C] = x.to(torch.bfloat16)
+    return out
+
+
+def _roi_align_fp64(feat, boxes, scale, images):
+    """torchvision roi_align(aligned=True) with one sample per bin, output size = the map's, in fp64: feat [B, h, w, C],
+    boxes [T, 4] (x1, y1, x2, y2), box t samples image images[t]"""
+    _, h, w, C = feat.shape
+
+    def taps(c, size):
+        # roi_align's bilinear_interpolate: outside [-1, size] -> 0; clamp at 0; the last row / column has no neighbour
+        valid = (c >= -1) & (c <= size)
+        c = c.clamp_min(0)
+        lo = c.floor().long().clamp_max(size - 1)
+        edge = c.floor() >= size - 1
+        hi = torch.where(edge, lo, lo + 1)
+        fr = torch.where(edge, torch.zeros_like(c), c - lo)
+        return lo, hi, fr, valid
+    out = []
+    for t in range(boxes.shape[0]):
+        x1, y1, x2, y2 = (boxes[t].double() * scale - 0.5).tolist()
+        ys = y1 + (torch.arange(h, dtype=torch.float64) + 0.5) * ((y2 - y1) / h)
+        xs = x1 + (torch.arange(w, dtype=torch.float64) + 0.5) * ((x2 - x1) / w)
+        yl, yh, fy, vy = taps(ys, h)
+        xl, xh, fx, vx = taps(xs, w)
+        f = feat[images[t]].double()
+        fy, fx = fy.view(-1, 1, 1), fx.view(1, -1, 1)
+        v = (1 - fy) * ((1 - fx) * f[yl][:, xl] + fx * f[yl][:, xh]) + fy * ((1 - fx) * f[yh][:, xl] + fx * f[yh][:, xh])
+        out.append(v * (vy.view(-1, 1, 1) & vx.view(1, -1, 1)))
+    return torch.stack(out)
+
+
+# (x1, y1, x2, y2) at scale 0.5 on an 8 x 16 map: dyadic, so every sample coordinate is exact in fp32 and fp64
+ROI_EDGE_BOXES = [
+    [-2.0, -2.0, 30.0, 14.0],       # first samples exactly at -1
+    [-1.5, 0.0, 30.5, 16.0],        # x samples in (-1, 0), y exactly at 0
+    [2.0, 2.0, 34.0, 18.0],         # samples at size - 1 and exactly at size
+    [1.0, 1.0, 41.0, 21.0],         # samples beyond size: zero
+    [-4.0, -3.5, 28.0, 4.5],        # samples below -1: zero; then exactly -1
+    [10.25, 3.5, 27.75, 12.25],     # fractional bins
+    [0.75, 1.25, 31.5, 15.0],
+]
+
+
+@pytest.mark.parametrize('f32', [False, True], ids=['bf16', 'fp32'])
+def test_roi_crop_zoom_batched_edges_poisoned(cuda, f32):
+    import ctypes
+    from patchfusion_b200 import ops
+    g = _gen(11)
+    B, h, w, C, ld, out_ld = 3, 8, 16, 20, 40, 48
+    boxes = torch.tensor(ROI_EDGE_BOXES, device=cuda)
+    T = boxes.shape[0]
+    images = [2, 0, 1, 1, 2, 0, 1]
+    tile_image = torch.tensor(images, dtype=torch.int32, device=cuda)
+    if f32:                 # the coarse depth: [B, h, w] fp32, one channel; NaN in the image past the batch
+        x = torch.rand(B, h, w, 1, device=cuda, generator=g) * 80
+        feat = torch.cat([x[..., 0], torch.full((1, h, w), float('nan'), device=cuda)]).contiguous()
+        out = torch.full((T + 1, h, w), SENTINEL, device=cuda)
+        ops.call('pf_roi_crop_zoom_batched', feat, 1, h, w, 1, 1, tile_image, boxes, T, ctypes.c_float(0.5), out, 1, 0,
+                 ops.stream_ptr())
+        got, xin = out[:T, ..., None].double(), x.double()
+    else:
+        x = torch.randn(B, h, w, C, device=cuda, generator=g) * 4
+        feat = _poisoned_nhwc(x, C, ld)
+        out = torch.full((T + 1, h, w, out_ld), SENTINEL, dtype=torch.bfloat16, device=cuda)
+        ops.call('pf_roi_crop_zoom_batched', feat, 0, h, w, ops.pad_to(C, 8), ld, tile_image, boxes, T,
+                 ctypes.c_float(0.5), out, out_ld, 0, ops.stream_ptr())
+        got, xin = out[:T, ..., :C].double(), rb(x).double()
+        assert (out[:T, ..., C:ops.pad_to(C, 8)] == 0).all(), 'pad channels [C, pad8(C)) not zero'
+        assert (out[:T, ..., ops.pad_to(C, 8):] == SENTINEL).all(), 'columns past pad8(C) written'
+    assert (out[T:] == SENTINEL).all(), 'wrote past the last box'
+    ref = _roi_align_fp64(xin.cpu(), boxes.cpu(), 0.5, images).to(cuda)
+    assert (ref == 0).any() and (ref != 0).any()
+    err = (got - ref).abs()
+    if f32:
+        tol = 1e-6 * xin.abs().max().item()
+    else:
+        # 1 bf16 ulp, plus the fp32 blend's own rounding where the value cancels to near zero
+        tol = torch.pow(2.0, torch.floor(torch.log2(ref.abs().clamp_min(2.0 ** -126))) - 7) + 2.0 ** -22 * xin.abs().max()
+    bad = (err > tol).nonzero()
+    assert bad.numel() == 0, '%d values off by more than %s, first at %s: got %r want %r' % (
+        bad.shape[0], 'the bound' if f32 else '1 bf16 ulp', bad[0].tolist(), got[tuple(bad[0])].item(),
+        ref[tuple(bad[0])].item())
+    print('roi crop-zoom %s: %d boxes at the roi_align edges, max |err| %.3e' % ('fp32' if f32 else 'bf16', T,
+                                                                               err.max().item()))
+
+
+def test_maxpool2_odd_poisoned(cuda):
+    """odd H and W: the last row and column are not read (floor mode); they, the pad columns and the image past the
+    batch hold 1e30, which wins any max it reaches"""
+    from patchfusion_b200 import ops
+    g = _gen(12)
+    B, H, W, C, ld, out_ld = 2, 13, 17, 20, 40, 32
+    x = torch.randn(B, H, W, C, device=cuda, generator=g)
+    x[:, H - 1] = 1e30
+    x[:, :, W - 1] = 1e30
+    feat = _poisoned_nhwc(x, C, ld, fill=1e30)
+    out = torch.full((B + 1, H // 2, W // 2, out_ld), SENTINEL, dtype=torch.bfloat16, device=cuda)
+    ops.call('pf_maxpool2', feat, B, H, W, ops.pad_to(C, 8), ld, out, out_ld, ops.stream_ptr())
+    ref = F.max_pool2d(rb(x).permute(0, 3, 1, 2), 2).permute(0, 2, 3, 1)
+    assert torch.equal(out[:B, ..., :C].float(), ref)
+    assert (out[:B, ..., C:ops.pad_to(C, 8)] == 0).all()
+    assert (out[:B, ..., ops.pad_to(C, 8):] == SENTINEL).all() and (out[B:] == SENTINEL).all()
+
+
+def test_im2col_3x3_s2_odd_poisoned(cuda):
+    from patchfusion_b200 import ops
+    g = _gen(13)
+    B, H, W, C, ld = 2, 13, 17, 24, 40
+    x = torch.randn(B, H, W, C, device=cuda, generator=g)
+    feat = _poisoned_nhwc(x, C, ld)
+    OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    rows = B * OH * OW
+    out = torch.full((rows + 4, 9 * C), SENTINEL, dtype=torch.bfloat16, device=cuda)
+    ops.call('pf_im2col_3x3_s2', feat, B, H, W, C, ld, out, ops.stream_ptr())
+    ref = F.unfold(rb(x).permute(0, 3, 1, 2), 3, padding=1, stride=2)          # [B, C * 9, OH * OW], (c, tap)
+    ref = ref.view(B, C, 9, OH * OW).permute(0, 3, 2, 1).reshape(rows, 9 * C)
+    assert torch.equal(out[:rows].float(), ref)
+    assert (out[rows:] == SENTINEL).all()
+
+
+def test_pack_unet_input_wide_poisoned(cuda):
+    """ld 16: channels 0-4 are the bf16 roundings, 5-7 zero, [8, 16) and the tile past T keep the sentinel; the inputs'
+    tile past T is NaN"""
+    from patchfusion_b200 import ops
+    g = _gen(14)
+    T, H, W, ld = 3, 13, 17, 16
+    nan = float('nan')
+    cd, fd = torch.full((T + 1, H, W), nan, device=cuda), torch.full((T + 1, H, W), nan, device=cuda)
+    rgb = torch.full((T + 1, 3, H, W), nan, device=cuda)
+    cd[:T], fd[:T] = torch.rand(T, H, W, device=cuda, generator=g) * 80, torch.rand(T, H, W, device=cuda, generator=g) * 80
+    rgb[:T] = torch.rand(T, 3, H, W, device=cuda, generator=g)
+    u = torch.full((T + 1, H, W, ld), SENTINEL, dtype=torch.bfloat16, device=cuda)
+    ops.call('pf_pack_unet_input', cd, fd, rgb, T, H, W, u, ld, ops.stream_ptr())
+    ref = torch.cat([cd[:T, None], fd[:T, None], rgb[:T]], 1).permute(0, 2, 3, 1).to(torch.bfloat16)
+    assert torch.equal(u[:T, ..., :5], ref)
+    assert (u[:T, ..., 5:8] == 0).all()
+    assert (u[:T, ..., 8:] == SENTINEL).all() and (u[T:] == SENTINEL).all()
+
+
+def test_f32_to_bf16_rounding(cuda):
+    """round to nearest even, as torch's conversion: ties both ways, +-0, subnormals (and their ties), the overflow
+    to inf past the largest bf16, +-inf; NaN stays NaN"""
+    from patchfusion_b200 import ops
+    g = _gen(15)
+    p = lambda e: 2.0 ** e                                                      # noqa: E731
+    special = [1 + p(-8), 1 + 3 * p(-8), 1 + p(-8) + p(-20), -(1 + p(-8)), -(1 + 3 * p(-8)), 0.0, -0.0,
+               p(-130), p(-133), p(-134), 3 * p(-134), -3 * p(-134), p(-149), p(-126) - p(-149), 1e-40,
+               (2 - p(-8)) * p(127), (2 - p(-8) - p(-20)) * p(127), 3.4028234663852886e38, -3.4028234663852886e38,
+               float('inf'), float('-inf'), 65504.0, 1.0 / 3]
+    x = torch.cat([torch.tensor(special, device=cuda),
+                   torch.randn(100003, device=cuda, generator=g) * torch.pow(10.0, torch.randint(
+                       -30, 30, (100003,), device=cuda, generator=g).float()),
+                   torch.tensor([float('nan'), -float('nan')], device=cuda)])
+    n = x.numel()
+    out = torch.full((n + 64,), SENTINEL, dtype=torch.bfloat16, device=cuda)
+    ops.call('pf_f32_to_bf16', x, n, out, ops.stream_ptr())
+    want = x.to(torch.bfloat16)
+    got = out[:n]
+    assert torch.isnan(got[-2:]).all(), 'NaN input must stay NaN'
+    k = n - 2
+    bad = (got[:k].view(torch.int16) != want[:k].view(torch.int16)).nonzero()
+    assert bad.numel() == 0, '%d values differ, first %r -> %r (want %r)' % (
+        bad.shape[0], x[bad[0]].item(), got[bad[0]].item(), want[bad[0]].item())
+    assert (out[n:] == SENTINEL).all()
+
+
 def test_swin_helpers(cuda):
     from patchfusion_b200 import ops
     g = _gen(6)
