@@ -11,12 +11,41 @@ libpf_b200 (sm_90a) through `Engine(parts=(branch,))`.  There is no CPU path: ca
 
 Two reference behaviours differ from `PatchFusion` and are kept: rN runs N `random_tile` calls of process_num tiles
 each (BP:407-410; PatchFusion runs N // process_num), and the fine target returns an empty info dict (BP:412-414).
+
+Calibrated FP8 (an extension; the reference has no such keys): `branch_vit_precision` / `branch_dpt_precision` ('bf16'
+default, or 'fp8_static') run the branch's DINOv2 qkv / fc1 / fc2 linears and its 19 covered DPT convs on E4M3 operands,
+as PatchFusion's `vit_precision` / `dpt_precision` do for its branches.  Their tables `branch_vit_fp8_amax` /
+`branch_dpt_fp8_amax` use PatchFusion's names for this branch ('<target>.<i>.<qkv|fc1|fc2>', '<target>.<conv>'), so
+the `fine.*` entries of a PatchFusion table are a fine baseline's table and the other way round;
+`BaselinePretrain.calibrate_fp8` fills them.  The tables are configuration: the state dict does not change.
+PatchFusion's own keys (fusion_precision, vit_precision, dpt_precision and their tables) are accepted and ignored.
 """
+import math
+import os
+
 import torch
 import torch.nn as nn
 
 from .model import AttrDict, Resize, TiledModel
-from .params import _get, branch_layout, synthetic_state_dict
+from .params import _get, branch_layout, dpt_fp8_amax, dpt_fp8_layers, dpt_precision, synthetic_state_dict, \
+    vit_fp8_amax, vit_fp8_layers, vit_precision
+
+
+FP8_KEYS = ('branch_vit_precision', 'branch_vit_fp8_amax', 'branch_dpt_precision', 'branch_dpt_fp8_amax')
+
+
+def save_baseline(model, cfg, out_dir, name):
+    """Write `model` as the pair `tools/test.py DIR/<name>.py --ckp-path DIR/<name>.pth` evaluates: the config file of
+    `cfg` (a load_config dict) whose model dict carries the model's FP8 keys, and {'model_state_dict':
+    get_save_dict()}, the checkpoint format the reference's BaselinePretrain reads.  Returns the two paths."""
+    from .config import save_config
+    os.makedirs(out_dir, exist_ok=True)
+    cfg = dict(cfg)
+    cfg['model'] = dict(cfg['model'], **{k: getattr(model, k) for k in FP8_KEYS})
+    paths = os.path.join(out_dir, name + '.py'), os.path.join(out_dir, name + '.pth')
+    save_config(cfg, paths[0])
+    torch.save({'model_state_dict': {k: v.detach().cpu() for k, v in model.get_save_dict().items()}}, paths[1])
+    return paths
 
 
 def _attr(cfg):
@@ -29,12 +58,14 @@ class BaselinePretrain(TiledModel):
     def __init__(self, coarse_branch, fine_branch, sigloss, min_depth, max_depth, image_raw_shape=(2160, 3840),
                  patch_process_shape=(384, 512), patch_split_num=(4, 4), target='coarse', coarse_branch_zoe=None,
                  fusion_precision=None, fusion_fp8_amax=None, vit_precision=None, vit_fp8_amax=None,
-                 dpt_precision=None, dpt_fp8_amax=None):
+                 dpt_precision=None, dpt_fp8_amax=None, branch_vit_precision='bf16', branch_vit_fp8_amax=None,
+                 branch_dpt_precision='bf16', branch_dpt_fp8_amax=None):
         nn.Module.__init__(self)
         # fusion_precision selects the compute type of PatchFusion's Guided-Fusion U-Net and fusion_fp8_amax holds its
         # calibrated FP8 input scales; this model has no fusion stage, so a config that carries the keys (any value)
         # builds and packs exactly as without them.  vit_precision / vit_fp8_amax and dpt_precision / dpt_fp8_amax
-        # (PatchFusion's FP8 ViT encoders and DPT decoders) are ignored the same way: FP8 baselines are not built.
+        # (PatchFusion's FP8 ViT encoders and DPT decoders) are ignored the same way, so a PatchFusion config's values
+        # never change a baseline: this model's FP8 switches are the branch_* keys.
         del fusion_precision, fusion_fp8_amax, vit_precision, vit_fp8_amax, dpt_precision, dpt_fp8_amax
         # patch_process_shape is deliberately not checked against the 14-px patch here: the shipped coarse configs
         # keep the (384, 512) default, and the reference fails only when a forward runs at a non-multiple of 14
@@ -57,10 +88,32 @@ class BaselinePretrain(TiledModel):
                 self.branch = target
                 self._build_tree(branch_layout(cfg, target + '_branch.'))
                 self.resizer = Resize(self.patch_process_shape[1], self.patch_process_shape[0], ensure_multiple_of=14)
+        self.branch_vit_precision = branch_vit_precision
+        self.branch_vit_fp8_amax = branch_vit_fp8_amax
+        self.branch_dpt_precision = branch_dpt_precision
+        self.branch_dpt_fp8_amax = branch_dpt_fp8_amax
+        self._fp8_cfg()                     # ValueError on an unknown precision or a malformed table
         self._runtime_init()
         self._hook_invalidate()
         if self.branch is not None:
             self._init_constant_buffers(_get(self._branch_cfg(), 'n_bins', 64))
+
+    def _fp8_cfg(self):
+        """The validated FP8 keys as the engine config of this branch (PatchFusion's key names, this branch's table
+        names): {} for the bf16 default, so the default engine is the one built without the keys."""
+        keys = {k: getattr(self, k) for k in FP8_KEYS}
+        keys.update(coarse_branch=self.coarse_branch_cfg, fine_branch=self.fine_branch_cfg)
+        own = (self.branch,) if self.branch is not None else ()
+        out = {}
+        if vit_precision(keys, 'branch_vit_precision') == 'fp8_static':
+            out.update(vit_precision='fp8_static', vit_fp8_amax=vit_fp8_amax(keys, 'branch_vit_fp8_amax', own))
+        else:
+            vit_fp8_amax(keys, 'branch_vit_fp8_amax', own)
+        if dpt_precision(keys, 'branch_dpt_precision') == 'fp8_static':
+            out.update(dpt_precision='fp8_static', dpt_fp8_amax=dpt_fp8_amax(keys, 'branch_dpt_fp8_amax', own))
+        else:
+            dpt_fp8_amax(keys, 'branch_dpt_fp8_amax', own)
+        return out
 
     def _branch_cfg(self):
         return self.coarse_branch_cfg if self.branch == 'coarse' else self.fine_branch_cfg
@@ -90,21 +143,82 @@ class BaselinePretrain(TiledModel):
     # ------------------------------------------------------------------ engine plumbing
     def engine(self, shape=None):
         """The packed branch at processing size `shape` (default patch_process_shape).  A call at another size
-        re-packs: the pos-embed resample depends on it."""
+        re-packs: the pos-embed resample depends on it.  The FP8 tables are read from the model's keys on every call: a
+        changed table re-points the stage and drops the graphs captured with the old scales."""
         from .engine import Engine
         if self.branch is None:
             raise NotImplementedError('no branch is built for target %r' % (self.target,))
         P = tuple(self.patch_process_shape if shape is None else shape)
-        if self._engine is not None and self._engine.P != P:
+        fp8 = self._fp8_cfg()
+        eng = self._engine
+        if eng is not None and (eng.P != P or (eng.vit_fp8_static, eng.dpt_fp8_static) !=
+                                ('vit_precision' in fp8, 'dpt_precision' in fp8)):
             self.invalidate()
         if self._engine is None:
             p = next(self.parameters())
             if not p.is_cuda:
                 raise RuntimeError('BaselinePretrain (H100): the hot path runs on libpf_b200 only; move the model to a '
                                    'CUDA device (there is no CPU fallback)')
-            cfg = {'patch_process_shape': P, self.branch + '_branch': self._branch_cfg()}
+            cfg = dict(fp8, patch_process_shape=P, **{self.branch + '_branch': self._branch_cfg()})
             self._engine = Engine(cfg, self.state_dict(), p.device, parts=(self.branch,))
+        else:
+            if eng.vit_fp8_static and fp8['vit_fp8_amax'] != eng.vit_amax:
+                eng.set_vit_fp8_amax(fp8['vit_fp8_amax'])
+                self._graphs = {}
+            if eng.dpt_fp8_static and fp8['dpt_fp8_amax'] != eng.dpt_amax:
+                eng.set_dpt_fp8_amax(fp8['dpt_fp8_amax'])
+                self._graphs = {}
         return self._engine
+
+    def _check_tables(self, eng):
+        """an 'fp8_static' branch without its calibration table refuses to run (calibration runs it in bf16)"""
+        if eng.calib is not None:
+            return
+        for on, table, key in ((eng.vit_fp8_static, eng.vit_amax, 'vit'), (eng.dpt_fp8_static, eng.dpt_amax, 'dpt')):
+            if on and table is None:
+                raise RuntimeError("branch_%s_precision 'fp8_static' needs the calibrated input scales `branch_%s_fp8_amax`: "
+                                   "run BaselinePretrain.calibrate_fp8 (or tools/calibrate_fp8.py) first" % (key, key))
+
+    @torch.no_grad()
+    def calibrate_fp8(self, image_lr, image_hr, cai_mode='m1', process_num=4, tile_cfg=None, reset=False):
+        """Post-training calibration of the 'fp8_static' branch: runs forward(mode='infer') on the given images (the
+        same arguments; the coarse target reads image_lr, one batch at its own size, the fine target the tiles of
+        image_hr, batches, mixed geometry and rN modes drawing from `random` included) with the branch in bf16 on this
+        model's panels, and takes, for each E4M3 ViT linear and each E4M3 DPT conv, the maximum over all images and
+        tiles of its input's amax.  Each switched-on table is merged by max into `branch_vit_fp8_amax` /
+        `branch_dpt_fp8_amax` (reset=True starts from empty tables).  Returns the ViT table, else the DPT table.  Runs
+        eagerly: no graph of it is kept, and the graphs of earlier forwards are dropped."""
+        fp8 = self._fp8_cfg()
+        vit, dpt = 'vit_precision' in fp8, 'dpt_precision' in fp8
+        if not vit and not dpt:
+            raise ValueError("calibrate_fp8 needs branch_vit_precision or branch_dpt_precision 'fp8_static' (this "
+                             "model: %r, %r)" % (self.branch_vit_precision, self.branch_dpt_precision))
+        # the coarse target runs at image_lr's size: pack there first, so the forward keeps this engine
+        eng = self.engine(tuple(image_lr.shape[-2:]) if self.target == 'coarse' and torch.is_tensor(image_lr) else None)
+        eng.calib = {}
+        graphs, self.use_cuda_graphs = self.use_cuda_graphs, False
+        try:
+            self.forward('infer', image_lr, image_hr, tile_cfg=tile_cfg, cai_mode=cai_mode, process_num=process_num)
+            found = {k: v.item() for k, v in eng.calib.items()}
+        finally:
+            eng.calib = None
+            self.use_cuda_graphs = graphs
+            self._graphs = {}
+        cfg = {'coarse_branch': self.coarse_branch_cfg, 'fine_branch': self.fine_branch_cfg}
+        own = (self.branch,)
+        for on, key, names, check in ((vit, 'branch_vit_fp8_amax', vit_fp8_layers(cfg, own), vit_fp8_amax),
+                                      (dpt, 'branch_dpt_fp8_amax', dpt_fp8_layers(cfg, own), dpt_fp8_amax)):
+            if not on:
+                continue
+            missing = [k for k in names if k not in found]
+            if missing:
+                raise RuntimeError('calibrate_fp8: no input amax for %s' % missing)
+            table = {} if reset else dict(getattr(self, key) or {})
+            for k in names:
+                table[k] = max(table.get(k, 0.0), found[k]) if not math.isnan(found[k]) else found[k]
+            setattr(self, key, check(dict(cfg, **{key: table}), key, own))      # ValueError on NaN / inf
+        self.engine(eng.P)
+        return dict(self.branch_vit_fp8_amax if vit else self.branch_dpt_fp8_amax)
 
     # ------------------------------------------------------------------ coarse target
     def _coarse_infer(self, image_lr):
@@ -114,6 +228,7 @@ class BaselinePretrain(TiledModel):
         assert h % 14 == 0, 'Input image height %d is not a multiple of patch height 14' % h
         assert w % 14 == 0, 'Input image width %d is not a multiple of patch width 14' % w
         eng = self.engine((h, w))
+        self._check_tables(eng)
         x = eng.buf('in.image_lr', (B, 3, h, w), torch.float32)
         x.copy_(image_lr)
         out = eng.buf('out.depth', (B, h, w), torch.float32)
@@ -188,6 +303,7 @@ class BaselinePretrain(TiledModel):
         assert len(image_hr) >= 1
         self._check_shard(shard, group)
         eng = self.engine()
+        self._check_tables(eng)
 
         def compute(phase, img, geom, tiles, sh, plan):
             return self._compute_phase(eng, phase, img, geom, tiles, process_num, sh)

@@ -6,6 +6,7 @@ then the file itself: a child key overrides, nested dicts merge recursively, lis
 The result is an `AttrDict` (attribute access, as the reference's code reads `cfg.val_dataloader.dataset`)."""
 import copy
 import os
+import pprint
 import runpy
 import types
 
@@ -40,6 +41,29 @@ def _file_dict(path):
 def load_config(path):
     """Config dict of a reference-format config file, `_base_` chains resolved."""
     return AttrDict(_file_dict(path))
+
+
+def _plain(v):
+    if isinstance(v, dict):
+        return {k: _plain(x) for k, x in v.items()}
+    if isinstance(v, (list, tuple)):
+        return type(v)(_plain(x) for x in v)
+    return v
+
+
+def save_config(cfg, path):
+    """Write cfg (a load_config dict, `_base_` already merged) as a self-contained config file that load_config reads
+    back equal: one `key = <literal>` per top-level key.  ValueError for a value without such a literal."""
+    cfg = _plain(dict(cfg))
+    text = ''.join('%s = %s\n' % (k, pprint.pformat(v, width=120, sort_dicts=False)) for k, v in cfg.items())
+    with open(path, 'w') as f:
+        f.write(text)
+    try:
+        back = _plain(dict(load_config(path)))
+    except Exception as e:
+        raise ValueError('save_config: %s does not load back (%r)' % (path, e))
+    if back != cfg:
+        raise ValueError('save_config: %s loads back as a different config' % path)
 
 
 def _parse_int_float_bool(v):

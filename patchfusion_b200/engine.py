@@ -79,15 +79,18 @@ class Engine:
         self.W = {}
         self._pack_all()
         self.sd = None   # fp32 originals are no longer needed on the device
-        self.c_branch = {b: self._c_branch(b) for b in ('coarse', 'fine') if b in self.parts}
+        # the branches this engine packs: both for PatchFusion, the built one for a single-branch model, whose config
+        # (and calibration tables) name that branch only
+        self.branches = tuple(b for b in ('coarse', 'fine') if b in self.parts)
+        self.c_branch = {b: self._c_branch(b) for b in self.branches}
         self.c_branch_bf16 = dict(self.c_branch)
         self.vit_amax = None
         self.dpt_amax = None
         self._branch_amax = {}
         if self.vit_fp8_static:
-            self.set_vit_fp8_amax(vit_fp8_amax(config))
+            self.set_vit_fp8_amax(vit_fp8_amax(config, branches=self.branches))
         if self.dpt_fp8_static:
-            self.set_dpt_fp8_amax(dpt_fp8_amax(config))
+            self.set_dpt_fp8_amax(dpt_fp8_amax(config, branches=self.branches))
         self.c_fusion = self._c_fusion() if 'fusion' in self.parts else None
         # 'fp8_static': c_fusion carries the calibrated input amax of each FP8 conv (set_fp8_amax); c_fusion_tiles is the
         # same stage with per-tile scales, which calibration runs.  `calib` (a dict while PatchFusion.calibrate_fp8 runs)
@@ -379,14 +382,14 @@ class Engine:
             self.vit_amax, self.c_branch = None, dict(self.c_branch_bf16)
             return
         self.vit_amax = dict(table)
-        self._set_branch_amax(vit_fp8_layers(self.cfg), self.vit_amax, 'vit')
+        self._set_branch_amax(vit_fp8_layers(self.cfg, self.branches), self.vit_amax, 'vit')
 
     def set_dpt_fp8_amax(self, table):
         """dpt_precision 'fp8_static': the calibrated input amax of the decoders' DPT_FP8_CONVS ({name of
         dpt_fp8_layers: float}, validated), or None (no table: the branches refuse to run, calibration still can).  Read
         when a stage is issued, so graphs captured before a change must be dropped (PatchFusion.engine does)."""
         self.dpt_amax = dict(table) if table is not None else None
-        self._set_branch_amax(dpt_fp8_layers(self.cfg), self.dpt_amax, 'dpt')
+        self._set_branch_amax(dpt_fp8_layers(self.cfg, self.branches), self.dpt_amax, 'dpt')
 
     def _set_branch_amax(self, names, table, kind):
         """re-points c_branch at the current ViT and DPT tables (kind: which of them `table` is)"""

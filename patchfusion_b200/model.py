@@ -214,7 +214,11 @@ class TiledModel(ParamTree):
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             n0 = lib.launch_count()
-            with torch.cuda.graph(g):
+            # thread-local capture: only this thread is barred from unsafe CUDA calls while it captures.  Other threads
+            # keep working; Tester's PNG writer, for one, waits on the previous image's copy events while the next
+            # image's forward captures its graphs.  In the default global mode that wait fails and invalidates the
+            # capture.
+            with torch.cuda.graph(g, capture_error_mode='thread_local'):
                 fn()
             self._graphs[key] = (g, lib.launch_count() - n0, eng.generation)
             return None

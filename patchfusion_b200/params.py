@@ -83,46 +83,56 @@ VIT_PRECISIONS = ('bf16', 'fp8_static')
 VIT_FP8_LINEARS = ('qkv', 'fc1', 'fc2')
 
 
-def vit_precision(config):
+BRANCHES = ('coarse', 'fine')
+
+
+def vit_precision(config, key='vit_precision'):
     """Top-level `vit_precision`: what the qkv, fc1 and fc2 linears of both branches' DINOv2 encoders compute in.
     'bf16' (default), or 'fp8_static': E4M3 operands with one calibrated scale per linear input (`vit_fp8_amax`,
-    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision."""
-    p = _get(config, 'vit_precision', 'bf16')
+    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision.  key: the config key to
+    read (BaselinePretrain's is 'branch_vit_precision')."""
+    p = _get(config, key, 'bf16')
     if p not in VIT_PRECISIONS:
-        raise ValueError("vit_precision should be one of 'bf16', 'fp8_static'")
+        raise ValueError("%s should be one of 'bf16', 'fp8_static'" % key)
     return p
 
 
-def vit_fp8_layers(config):
-    """The names of vit_fp8_amax: '{coarse|fine}.{i}.{qkv|fc1|fc2}' for every block i of each branch's encoder"""
+def vit_fp8_layers(config, branches=BRANCHES):
+    """The names of vit_fp8_amax: '{coarse|fine}.{i}.{qkv|fc1|fc2}' for every block i of each branch's encoder
+    (branches: the branches to list, in this order; a single-branch model lists its own)"""
     names = []
-    for b in ('coarse', 'fine'):
+    for b in branches:
         depth = branch_hparams(_get(config, b + '_branch'))['depth']
         names += ['%s.%d.%s' % (b, i, k) for i in range(depth) for k in VIT_FP8_LINEARS]
     return tuple(names)
 
 
-def vit_fp8_amax(config):
-    """Top-level `vit_fp8_amax`: the calibrated amax of each E4M3 ViT linear's input, {name of vit_fp8_layers: float
-    >= 0} with exactly those 6 * depth names, or None when the config has no table.  Anything else raises ValueError."""
-    t = _get(config, 'vit_fp8_amax', None)
+def _amax_table(t, key, names, what):
+    """{name: float >= 0} with exactly `names`, or None for None; anything else raises ValueError"""
     if t is None:
         return None
-    names = vit_fp8_layers(config)
     if not isinstance(t, dict):
-        raise ValueError('vit_fp8_amax should be a dict of the %d ViT linear names to their input amax' % len(names))
+        raise ValueError('%s should be a dict of the %d %s names to their input amax' % (key, len(names), what))
     known = set(names)
     missing = [k for k in names if k not in t]
     unknown = sorted(str(k) for k in t if k not in known)
     if missing or unknown:
-        raise ValueError('vit_fp8_amax: missing layers %s, unknown layers %s' % (missing, unknown))
+        raise ValueError('%s: missing layers %s, unknown layers %s' % (key, missing, unknown))
     out = {}
     for k in names:
         v = t[k]
         if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
-            raise ValueError('vit_fp8_amax[%r] = %r: a finite float >= 0 is required' % (k, v))
+            raise ValueError('%s[%r] = %r: a finite float >= 0 is required' % (key, k, v))
         out[k] = float(v)
     return out
+
+
+def vit_fp8_amax(config, key='vit_fp8_amax', branches=BRANCHES):
+    """Top-level `vit_fp8_amax`: the calibrated amax of each E4M3 ViT linear's input, {name of vit_fp8_layers: float
+    >= 0} with exactly those 6 * depth names (3 * depth for one branch), or None when the config has no table.
+    Anything else raises ValueError."""
+    t = _get(config, key, None)
+    return None if t is None else _amax_table(t, key, vit_fp8_layers(config, branches), 'ViT linear')
 
 
 DPT_PRECISIONS = ('bf16', 'fp8_static')
@@ -134,42 +144,28 @@ DPT_FP8_CONVS = tuple(['layer%d_rn' % i for i in range(1, 5)] +
                       ['refinenet4.resConfUnit2.conv%d' % k for k in (1, 2)] + ['output_conv1'])
 
 
-def dpt_precision(config):
+def dpt_precision(config, key='dpt_precision'):
     """Top-level `dpt_precision`: what the DPT decoders' covered 3x3 convs (DPT_FP8_CONVS) of both branches compute in.
     'bf16' (default), or 'fp8_static': E4M3 operands with one calibrated scale per conv input (`dpt_fp8_amax`,
-    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision and vit_precision."""
-    p = _get(config, 'dpt_precision', 'bf16')
+    PatchFusion.calibrate_fp8) and one per output channel.  Independent of fusion_precision and vit_precision.  key:
+    the config key to read (BaselinePretrain's is 'branch_dpt_precision')."""
+    p = _get(config, key, 'bf16')
     if p not in DPT_PRECISIONS:
-        raise ValueError("dpt_precision should be one of 'bf16', 'fp8_static'")
+        raise ValueError("%s should be one of 'bf16', 'fp8_static'" % key)
     return p
 
 
-def dpt_fp8_layers(config=None):
-    """The names of dpt_fp8_amax: '{coarse|fine}.<conv>' for every conv of DPT_FP8_CONVS, 38 in all"""
-    return tuple('%s.%s' % (b, n) for b in ('coarse', 'fine') for n in DPT_FP8_CONVS)
+def dpt_fp8_layers(config=None, branches=BRANCHES):
+    """The names of dpt_fp8_amax: '{coarse|fine}.<conv>' for every conv of DPT_FP8_CONVS, 38 in all (19 for one branch)"""
+    return tuple('%s.%s' % (b, n) for b in branches for n in DPT_FP8_CONVS)
 
 
-def dpt_fp8_amax(config):
+def dpt_fp8_amax(config, key='dpt_fp8_amax', branches=BRANCHES):
     """Top-level `dpt_fp8_amax`: the calibrated amax of each E4M3 DPT conv's input, {name of dpt_fp8_layers: float >= 0}
-    with exactly those 38 names, or None when the config has no table.  Anything else raises ValueError."""
-    t = _get(config, 'dpt_fp8_amax', None)
-    if t is None:
-        return None
-    names = dpt_fp8_layers(config)
-    if not isinstance(t, dict):
-        raise ValueError('dpt_fp8_amax should be a dict of the %d DPT conv names to their input amax' % len(names))
-    known = set(names)
-    missing = [k for k in names if k not in t]
-    unknown = sorted(str(k) for k in t if k not in known)
-    if missing or unknown:
-        raise ValueError('dpt_fp8_amax: missing layers %s, unknown layers %s' % (missing, unknown))
-    out = {}
-    for k in names:
-        v = t[k]
-        if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(v) or v < 0:
-            raise ValueError('dpt_fp8_amax[%r] = %r: a finite float >= 0 is required' % (k, v))
-        out[k] = float(v)
-    return out
+    with exactly those 38 names (19 for one branch), or None when the config has no table.  Anything else raises
+    ValueError."""
+    t = _get(config, key, None)
+    return None if t is None else _amax_table(t, key, dpt_fp8_layers(config, branches), 'DPT conv')
 
 
 def branch_hparams(branch_cfg):

@@ -9,6 +9,13 @@ evaluation reads them) and writes a save_pretrained directory whose config carri
 calibration table `fusion_fp8_amax`.  `tools/test.py <config.py> --ckp-path DIR` then evaluates the calibrated model.
 A config that selects dpt_precision 'fp8_static' (`--cfg-options model.config.dpt_precision=fp8_static`) gets the DPT
 decoders' table `dpt_fp8_amax` filled, written and printed too.
+
+A config whose model is a BaselinePretrain (the coarse-only / fine-only baselines, a .pth checkpoint) gets
+branch_vit_precision 'fp8_static' (and its branch_dpt_precision as the config or
+`--cfg-options model.branch_dpt_precision=fp8_static` selects it), is calibrated by BaselinePretrain.calibrate_fp8 on
+the same images, and is written as DIR/<config name>.py, the config with the tables in its model dict, and
+DIR/<config name>.pth, {'model_state_dict': ...}: `tools/test.py DIR/<config name>.py --ckp-path DIR/<config name>.pth`
+evaluates the calibrated baseline.
 """
 import argparse
 import json
@@ -22,7 +29,7 @@ import torch  # noqa: E402
 
 
 def main(argv=None):
-    p = argparse.ArgumentParser(description='Calibrate the static FP8 U-Net of a PatchFusion model')
+    p = argparse.ArgumentParser(description='Calibrate the static FP8 layers of a PatchFusion or BaselinePretrain model')
     p.add_argument('config')
     p.add_argument('--ckp-path', type=str, required=True)
     p.add_argument('--test-type', type=str, default='normal')
@@ -32,10 +39,13 @@ def main(argv=None):
     p.add_argument('--patch-split-num', nargs='+', default=[4, 4])
     p.add_argument('--cfg-options', nargs='+', default=None)
     p.add_argument('--num-images', type=int, required=True)
-    p.add_argument('--out', type=str, required=True, help='save_pretrained directory to write')
+    p.add_argument('--out', type=str, required=True,
+                   help='directory to write (a save_pretrained directory, or a baseline config + .pth)')
     args = p.parse_args(argv)
     from estimator.datasets import build_dataset
+    from estimator.models import build_model as build_from_cfg
     from patchfusion_b200 import imageio
+    from patchfusion_b200.baseline import BaselinePretrain, save_baseline
     from patchfusion_b200.config import load_config, merge_options, parse_options
     from patchfusion_b200.datasets import PreparedSamples
     from patchfusion_b200.evaluate import DATALOADERS, build_model, fix_random_seed
@@ -48,14 +58,24 @@ def main(argv=None):
     fix_random_seed(cfg.get('seed', 5621))
     device = torch.device('cuda', torch.cuda.current_device())
     src = build_model(cfg, args.ckp_path)
-    # the same weights in an 'fp8_static' model (the table starts empty: calibrate_fp8 fills it)
-    conf = dict(src.config.to_dict(), fusion_precision='fp8_static')
-    conf.pop('fusion_fp8_amax', None)
-    dpt = conf.get('dpt_precision', 'bf16') == 'fp8_static'     # the DPT decoders' table too
-    if dpt:
-        conf.pop('dpt_fp8_amax', None)
-    model = PatchFusion(conf)
-    model.load_state_dict(src.state_dict(), strict=True)
+    baseline = isinstance(src, BaselinePretrain)
+    if baseline:
+        # the same branch weights in a model with an 'fp8_static' ViT (tables start empty: calibrate_fp8 fills them)
+        conf = dict(cfg.model, branch_vit_precision='fp8_static')
+        dpt = conf.get('branch_dpt_precision', 'bf16') == 'fp8_static'
+        for k in ('branch_vit_fp8_amax', 'branch_dpt_fp8_amax'):
+            conf.pop(k, None)
+        model = build_from_cfg(conf)
+        model.load_dict(src.get_save_dict())
+    else:
+        # the same weights in an 'fp8_static' model (the table starts empty: calibrate_fp8 fills it)
+        conf = dict(src.config.to_dict(), fusion_precision='fp8_static')
+        conf.pop('fusion_fp8_amax', None)
+        dpt = conf.get('dpt_precision', 'bf16') == 'fp8_static'     # the DPT decoders' table too
+        if dpt:
+            conf.pop('dpt_fp8_amax', None)
+        model = PatchFusion(conf)
+        model.load_state_dict(src.state_dict(), strict=True)
     del src
     model = model.to(device).eval()
     dataset = build_dataset(cfg[DATALOADERS.get(args.test_type, 'val_dataloader')].dataset)
@@ -69,10 +89,18 @@ def main(argv=None):
                                     tile_cfg=tile_cfg)
     if table is None:
         raise SystemExit('calibrate_fp8: the dataset has no images')
-    model.save_pretrained(args.out)
-    out = dict(images=n, fusion_fp8_amax=table)
-    if dpt:
-        out['dpt_fp8_amax'] = dict(model.config['dpt_fp8_amax'])
+    if baseline:
+        name = os.path.splitext(os.path.basename(args.config))[0]
+        cfg['model'] = conf
+        save_baseline(model, cfg, args.out, name)
+        out = dict(images=n, branch_vit_fp8_amax=table)
+        if dpt:
+            out['branch_dpt_fp8_amax'] = dict(model.branch_dpt_fp8_amax)
+    else:
+        model.save_pretrained(args.out)
+        out = dict(images=n, fusion_fp8_amax=table)
+        if dpt:
+            out['dpt_fp8_amax'] = dict(model.config['dpt_fp8_amax'])
     print(json.dumps(out, indent=1))
     return table
 
