@@ -388,6 +388,35 @@ int pf_stitch_reduce(float* stack, int32_t world, int64_t n, void* stream);
 int pf_stitch_resize(const float* num, const float* den, int32_t H, int32_t W, int32_t OH, int32_t OW, float* num_out,
                      float* den_out, void* stream);
 
+/* ---- depth to 3D (external/zoedepth/utils/geometry.py) --------------------------------------------------------- */
+/* depth_to_points (geometry.py:39-72) of depth [H, W] fp32: points [H*W, 3] fp32, p = R M d K^-1 [x, y, 1]^T + t with
+ * K = get_intrinsics(H, W) (55 degree FOV, f = W / 2 / tan(27.5 deg), principal point (W/2, H/2); inv_f = fp32 1/f)
+ * and M = diag(-1, -1, 1).  rt_host (nullable: identity and zero): 12 host floats, R row-major then t.  image
+ * (nullable, with colors): planar RGB [3, H, W] fp32; colors [H*W, 3] uint8 = round-half-even(255 clamp(v, 0, 1)),
+ * NaN -> 0, written by the same pass. */
+int pf_depth_to_points(const float* depth, int32_t H, int32_t W, float inv_f, const float* rt_host, const float* image,
+                       float* points, uint8_t* colors, void* stream);
+/* Vertex mask [H, W] uint8 (H, W >= 2): 1 where d is finite, d > 0 and hypot(gy, gx) <= threshold, with (gy, gx) =
+ * np.gradient(d) in fp32 (central differences / 2 inside, one-sided differences at the borders). */
+int pf_depth_edge_mask(const float* depth, int32_t H, int32_t W, float threshold, uint8_t* mask, void* stream);
+/* create_triangles (geometry.py:75-98) with a vertex mask [h, w] (uint8 / bool, nonzero = set), in two calls with one
+ * read of the total between them.  Quads are row-major; quad q's triangles are (tl, bl, tr) then (br, tr, bl), and a
+ * triangle is kept when its three vertices are set.
+ * pf_mesh_quad_counts: flags [(h-1)(w-1)] uint8 (bit 0 / bit 1: first / second triangle kept) and block_offsets
+ * [ceil((h-1)(w-1) / PF_MESH_SCAN_BLOCK) + 1] int64: the exclusive offset of every block of PF_MESH_SCAN_BLOCK quads,
+ * then the total.  Deterministic (no atomics).
+ * pf_mesh_triangles: faces [n, 3] int32 in numpy boolean-indexing order; nothing is written at or past row `cap`.
+ * flags == NULL: every triangle, 2 (h-1)(w-1) rows (cap must hold them), block_offsets unused. */
+#define PF_MESH_SCAN_BLOCK 64
+int pf_mesh_quad_counts(const uint8_t* mask, int32_t h, int32_t w, uint8_t* flags, int64_t* block_offsets,
+                        void* stream);
+int pf_mesh_triangles(const uint8_t* flags, const int64_t* block_offsets, int32_t h, int32_t w, int32_t* faces,
+                      int64_t cap, void* stream);
+/* Binary little-endian PLY records, out 16-byte aligned: vertices 15 bytes each (float x, y, z; uchar r, g, b) from
+ * points [n, 3] fp32 and colors [n, 3] uint8; faces 13 bytes each (uchar 3; int32 a, b, c) from faces [n, 3] int32. */
+int pf_ply_pack_vertices(const float* points, const uint8_t* colors, int64_t n, uint8_t* out, void* stream);
+int pf_ply_pack_faces(const int32_t* faces, int64_t n, uint8_t* out, void* stream);
+
 
 /* ================================================================================================================
  * STAGE-LEVEL ENTRY POINTS (SURVEY.md §8b): the kernel sequences behind the reference's methods, issued by the

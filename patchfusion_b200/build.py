@@ -5,7 +5,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
-SOURCES = ['pf_api.cu', 'pf_gemm.cu', 'pf_attn.cu', 'pf_elem.cu', 'pf_post.cu', 'pf_eval.cu', 'pf_stage.cu']
+SOURCES = ['pf_api.cu', 'pf_gemm.cu', 'pf_attn.cu', 'pf_elem.cu', 'pf_post.cu', 'pf_eval.cu', 'pf_stage.cu', 'pf_geom.cu']
 LIB = os.path.join(HERE, os.environ.get('PF_B200_LIBNAME', 'libpf_b200.so'))
 EXTRA = os.environ.get('PF_B200_NVCC_EXTRA', '').split()
 ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']

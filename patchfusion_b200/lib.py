@@ -17,6 +17,7 @@ ACT_NONE, ACT_RELU, ACT_GELU, ACT_SOFTPLUS = 0, 1, 2, 3
 BINS_TYPES = {'softplus': 0, 'normed': 1, 'hybrid1': 2, 'hybrid2': 3}
 QUANT_PARTS = 32    # PF_QUANT_PARTS: partial maxima per tile of pf_quantize_e4m3_tiles
 SEED_NORMED, SEED_TO_UNIT = 1, 2
+MESH_SCAN_BLOCK = 64  # PF_MESH_SCAN_BLOCK: quads per block of pf_mesh_quad_counts' scan
 OPT_TMA_EPILOGUE, OPT_HALO_MULTICAST, OPT_GEMM_MULTICAST, OPT_FUSED_RESAMPLE, OPT_PDL, OPT_RESIZE_SEPARABLE = 0, 1, 2, 3, 4, 5
 
 
@@ -111,6 +112,12 @@ SIGNATURES = {
     'pf_stitch_finalize': [_p, _p, _ll, _p, _p],
     'pf_stitch_reduce': [_p, _i, _ll, _p],
     'pf_stitch_resize': [_p, _p, _i, _i, _i, _i, _p, _p, _p],
+    'pf_depth_to_points': [_p, _i, _i, _f, C.POINTER(C.c_float), _p, _p, _p, _p],
+    'pf_depth_edge_mask': [_p, _i, _i, _f, _p, _p],
+    'pf_mesh_quad_counts': [_p, _i, _i, _p, _p, _p],
+    'pf_mesh_triangles': [_p, _p, _i, _i, _p, _ll, _p],
+    'pf_ply_pack_vertices': [_p, _p, _ll, _p, _p],
+    'pf_ply_pack_faces': [_p, _ll, _p, _p],
 }
 EXPORTS = sorted(list(SIGNATURES) + ['pf_last_error', 'pf_version', 'pf_launch_count', 'pf_branch_workspace_bytes', 'pf_branch_forward',
                   'pf_g2l_workspace_bytes', 'pf_g2l_forward', 'pf_fusion_workspace_bytes', 'pf_fusion_forward',

@@ -399,3 +399,44 @@ def attractor_normed(A, nA, b_prev, flags, min_depth, max_depth, b_out, centers=
     _, PH, PW, nb = b_prev.shape
     call('pf_attractor_normed', A, A_ld, nA, b_prev, PH, PW, B, H, W, nb, flags, C.c_float(min_depth),
          C.c_float(max_depth), b_out, centers, stream_ptr())
+
+
+def depth_to_points(depth, inv_f, rt, image, points, colors=None):
+    """pf_depth_to_points: depth [.., H, W] fp32 -> points [H*W, 3] fp32; rt: 12 floats (R row-major, then t) or None
+    (identity, zero); image: planar RGB [.., 3, H, W] fp32 or None, whose colours go to colors [H*W, 3] uint8."""
+    H, W = depth.shape[-2:]
+    rt_c = None if rt is None else (C.c_float * 12)(*rt)
+    call('pf_depth_to_points', depth, H, W, C.c_float(inv_f), rt_c, image, points, colors, stream_ptr())
+
+
+def depth_edge_mask(depth, threshold, out):
+    """pf_depth_edge_mask: depth [.., H, W] fp32 -> out [H, W] (uint8 or bool storage), 1 where the vertex is kept."""
+    H, W = depth.shape[-2:]
+    call('pf_depth_edge_mask', depth, H, W, C.c_float(threshold), out, stream_ptr())
+
+
+def mesh_scan_blocks(h, w):
+    """blocks of pf_mesh_quad_counts' scan: `offsets` holds this many int64 offsets plus the total"""
+    return ((h - 1) * (w - 1) + lib.MESH_SCAN_BLOCK - 1) // lib.MESH_SCAN_BLOCK
+
+
+def mesh_quad_counts(mask, h, w, flags, offsets):
+    """pf_mesh_quad_counts: vertex mask [h, w] (uint8 / bool) -> kept-triangle flags [(h-1)(w-1)] uint8 and
+    offsets [mesh_scan_blocks(h, w) + 1] int64 (per-block output offsets, then the triangle count)."""
+    call('pf_mesh_quad_counts', mask, h, w, flags, offsets, stream_ptr())
+
+
+def mesh_triangles(flags, offsets, h, w, faces):
+    """pf_mesh_triangles: the kept triangles into faces [n, 3] int32 (flags None: all 2 (h-1)(w-1) of them); writes
+    nothing past faces.shape[0] rows."""
+    call('pf_mesh_triangles', flags, offsets, h, w, faces, C.c_int64(faces.shape[0]), stream_ptr())
+
+
+def ply_pack_vertices(points, colors, out):
+    """pf_ply_pack_vertices: points [n, 3] fp32 + colors [n, 3] uint8 -> out [15 n] uint8 PLY vertex records"""
+    call('pf_ply_pack_vertices', points, colors, C.c_int64(points.shape[0]), out, stream_ptr())
+
+
+def ply_pack_faces(faces, out):
+    """pf_ply_pack_faces: faces [n, 3] int32 -> out [13 n] uint8 PLY face records"""
+    call('pf_ply_pack_faces', faces, C.c_int64(faces.shape[0]), out, stream_ptr())
