@@ -532,7 +532,9 @@ typedef struct pf_fusion {
 typedef struct pf_map { void* ptr; int32_t B, H, W, C, ld; } pf_map;     /* NHWC bf16 activation */
 typedef struct pf_branch_out { float* depth; pf_map feats[6]; } pf_branch_out;   /* x_d0, r4, r3, r2, r1, out_conv */
 
-/* debug tap: called (synchronously, while enqueuing) after the named intermediate has been produced */
+/* debug tap: called (synchronously, while enqueuing) after the named intermediate has been produced.  The layer taps
+ * "L.<layer>.<part>" of the bf16 GEMMs and convs (<layer>: the engine's weight key) also name what a launch is about
+ * to read (in<s>, res1, res2, x), emitted just before it: a callback that copies on the stream sees those values. */
 typedef void (*pf_tap_fn)(void* user, const char* name, const void* ptr, int32_t is_f32, int64_t rows, int32_t cols,
                           int32_t ld);
 
@@ -545,7 +547,7 @@ int pf_branch_forward(const pf_branch* w, const float* images, int32_t B, void* 
  * image and image b equals its batch-1 result bit for bit. */
 size_t pf_g2l_workspace_bytes(const pf_fusion* w, const pf_map* coarse_feats);
 int pf_g2l_forward(const pf_fusion* w, const pf_map* coarse_feats, void* ws, size_t ws_bytes, pf_map* out,
-                   void* stream);
+                   pf_tap_fn tap, void* tap_user, void* stream);
 size_t pf_fusion_workspace_bytes(const pf_fusion* w, int32_t T, const pf_map* g2l_maps);
 /* crops planar fp32 [T,3,H,W]; boxes fp32 [T,4] (x1,y1,x2,y2 in patch_process units, device); fine_* = the fine
  * branch's outputs for the same T tiles; coarse_* / g2l_maps = the whole-image (batch 1) outputs; depth_out [T,H,W]. */

@@ -5,6 +5,7 @@
 // running the same code in "dry" mode (no launches).  Reference lines are cited at each step.
 #include <cuda_bf16.h>
 #include <math.h>
+#include <stdarg.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -31,7 +32,8 @@ struct Ctx {
   int err;
   pf_tap_fn tap; void* tap_user;
   int n_e4m3;           // FP8 convs issued so far (names their debug taps)
-  const char* lname;    // name of the U-Net conv being issued (FP8_LAYERS in params.py), for the calibration taps
+  const char* lname;    // name of the layer being issued (the engine's weight key), for the calibration and layer taps
+  char lbuf[48];
 
   void* alloc(size_t bytes) {
     off = (off + 255) & ~static_cast<size_t>(255);
@@ -54,6 +56,23 @@ struct Ctx {
   void chk(int rc) { if (rc && !err) err = rc; }
   void tap_out(const char* name, const void* ptr, int is_f32, long long rows, int cols, int ld) {
     if (tap && live()) tap(tap_user, name, ptr, is_f32, rows, cols, ld);
+  }
+  // names the next GEMM / conv (every call site names its layer, so no launch inherits another's name)
+  void name(const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(lbuf, sizeof(lbuf), fmt, ap);
+    va_end(ap);
+    lname = lbuf;
+  }
+  // layer tap "L.<lname>.<part>" of a bf16 GEMM / conv (tests/test_gpu_stage_layers.py checks each layer on exactly
+  // these inputs).  Taps issued before the launch (in<s>, res1, res2, x) are copied by the callback in stream order, so
+  // they hold what the kernel read.
+  bool ltaps() const { return tap != nullptr && lname != nullptr && live(); }
+  void ltap(const char* part, const void* ptr, int is_f32, long long rows, int cols, int ld) {
+    char nm[64];
+    snprintf(nm, sizeof(nm), "L.%s.%s", lname, part);
+    tap_out(nm, ptr, is_f32, rows, cols, ld);
   }
 };
 
@@ -95,6 +114,25 @@ static void gemm_desc_common(pf_gemm_desc& d, const pf_layer& L, const GemmOpt& 
   }
 }
 
+// layer taps around a bf16 launch: the residuals and the fp32 stream a gamma update accumulates into before it, the
+// outputs after it (out: the main store, out2: the ReLU copy, out3: the fused tail, vt: the qkv's V^T)
+static void ltap_pre(Ctx& c, const pf_layer& L, const GemmOpt& o, long long rows, const void* out, int out_ld) {
+  if (!c.ltaps()) return;
+  if (o.res1) c.ltap("res1", o.res1->p, 0, rows, L.N, o.res1->ld);
+  if (o.res2) c.ltap("res2", o.res2->p, 0, rows, L.N, o.res1->ld);
+  if (o.gamma) c.ltap("x", out, 1, rows, L.N, out_ld);
+}
+static void ltap_post(Ctx& c, const pf_layer& L, const GemmOpt& o, long long rows, const void* out, int out_f32,
+                      int out_ld) {
+  if (!c.ltaps()) return;
+  const int ps = L.ps > 1 ? L.ps : 1;
+  if (!o.skip_main)
+    c.ltap("out", out, out_f32, rows * ps * ps, ps > 1 ? L.ps_cout : (o.vt ? o.vt_col0 : L.N), out_ld);
+  if (o.relu_copy) c.ltap("out2", o.relu_copy->p, 0, rows, L.N, o.relu_copy->ld);
+  if (o.tail) c.ltap("out3", o.out3, 1, rows, L.n2, o.out3_ld);
+  if (o.vt) c.ltap("vt", o.vt, 0, rows / o.vt_seq * (L.N - o.vt_col0), o.vt_seq, o.vt_seq_pad);
+}
+
 // D[M, N] = A[M, K] W^T : A is a bf16 matrix with `cols` logical columns and row stride ld
 static void linear(Ctx& c, const pf_layer& L, const bf16* A, long long M, int cols, int ld, void* out, int out_f32,
                    int out_ld, const GemmOpt& o = GemmOpt()) {
@@ -106,7 +144,10 @@ static void linear(Ctx& c, const pf_layer& L, const bf16* A, long long M, int co
   d.M = static_cast<int32_t>(M);
   if (L.ps > 1) { d.NB = o.ps_B; d.H = o.ps_H; d.W = o.ps_W; }
   gemm_desc_common(d, L, o, out, out_f32, out_ld);
+  if (c.ltaps()) c.ltap("in0", A, 0, M, cols, ld);
+  ltap_pre(c, L, o, M, out, out_ld);
   c.chk(pf_gemm(&d, c.stream));
+  ltap_post(c, L, o, M, out, out_f32, out_ld);
 }
 
 // FP8 3x3 conv (a layer packed with pf_pack_weight_e4m3: fusion_precision 'fp8'): the sources are quantized with one
@@ -288,6 +329,16 @@ static void conv_dpt_e4m3(Ctx& c, const char* name, const pf_layer& L, const voi
   }
 }
 
+// layer taps "in<s>": a conv's sources as the kernel reads them (a fused-resample conv's at their own size)
+static void ltap_srcs(Ctx& c, const Map* const* srcs, int ns) {
+  if (!c.ltaps()) return;
+  for (int i = 0; i < ns; ++i) {
+    char p[8];
+    snprintf(p, sizeof(p), "in%d", i);
+    c.ltap(p, srcs[i]->p, 0, srcs[i]->rows(), srcs[i]->C, srcs[i]->ld);
+  }
+}
+
 // 3x3 / 1x1 conv over up to three channel-concatenated NHWC sources
 static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns, void* out, int out_f32, int out_ld,
                       const GemmOpt& o = GemmOpt()) {
@@ -315,7 +366,10 @@ static void conv_into(Ctx& c, const pf_layer& L, const Map* const* srcs, int ns,
   for (int i = 0; i < ns; ++i) { d.a_ptr[i] = srcs[i]->p; d.a_c[i] = pad_to(srcs[i]->C, 8); d.a_ld[i] = srcs[i]->ld; }
   d.NB = srcs[0]->B; d.H = srcs[0]->H; d.W = srcs[0]->W;
   gemm_desc_common(d, L, o, out, out_f32, out_ld);
+  ltap_srcs(c, srcs, ns);
+  ltap_pre(c, L, o, srcs[0]->rows(), out, out_ld);
   c.chk(pf_gemm(&d, c.stream));
+  ltap_post(c, L, o, srcs[0]->rows(), out, out_f32, out_ld);
 }
 
 // 3x3 conv whose sources are read THROUGH F.interpolate(mode='bilinear', align_corners=True) to (H, W): sources of
@@ -347,7 +401,10 @@ static Map conv_resampled(Ctx& c, const pf_layer& L, const Map* const* srcs, int
   }
   d.NB = srcs[0]->B; d.H = H; d.W = W;
   gemm_desc_common(d, L, o, out.p, 0, out.ld);
+  ltap_srcs(c, srcs, ns);
+  ltap_pre(c, L, o, out.rows(), out.p, out.ld);
   c.chk(pf_gemm(&d, c.stream));
+  ltap_post(c, L, o, out.rows(), out.p, 0, out.ld);
   return out;
 }
 
@@ -421,14 +478,18 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
                         float* depth_out) {
   const int B = x.B, nb = Hd.n_bins, E = Hd.bin_embedding_dim;
   // two-layer 1x1 MLP `_net` (localbins_layers.py:84-89,110-114, attractor.py:157-162)
-  auto mlp_bf16 = [&](const pf_layer& L0, const pf_layer& L2, const Map& src) -> Map {
+  // `mod`: the module's name in the engine's head weights (layer taps "L.head.<mod>.0|2")
+  auto mlp_bf16 = [&](const pf_layer& L0, const pf_layer& L2, const Map& src, const char* mod) -> Map {
     GemmOpt o0; o0.act = PF_ACT_RELU;
+    c.name("head.%s.0", mod);
     Map t = conv1(c, L0, src, o0);
+    c.name("head.%s.2", mod);
     return conv1(c, L2, t);
   };
-  auto mlp_f32 = [&](const pf_layer& L0, const pf_layer& L2, const Map& src, int act2) -> MapF {
+  auto mlp_f32 = [&](const pf_layer& L0, const pf_layer& L2, const Map& src, int act2, const char* mod) -> MapF {
     const int n_out = L0.n2 > 0 ? L0.n2 : L2.N;
     MapF o = c.mapf(B, src.H, src.W, n_out, pad_to(pad_to(n_out, 8), 32));
+    c.name("head.%s.0", mod);
     if (L0.n2 > 0) {       // narrow second layer fused into the first layer's epilogue
       GemmOpt g; g.act = PF_ACT_RELU; g.tail = true; g.act2 = act2; g.out3 = o.p; g.out3_ld = o.ld; g.skip_main = true;
       conv1(c, L0, src, g);
@@ -437,6 +498,7 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
       Map t = conv1(c, L0, src, o0);
       const Map* a[1] = {&t};
       GemmOpt g2; g2.act = act2;
+      c.name("head.%s.2", mod);
       conv_into(c, L2, a, 1, o.p, 1, o.ld, g2);
     }
     return o;
@@ -451,7 +513,8 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
   }
   const bool normed_seed = type == PF_BINS_NORMED || type == PF_BINS_HYBRID1;
   const bool normed_att = type == PF_BINS_NORMED || type == PF_BINS_HYBRID2;
-  MapF b_prev = mlp_f32(Hd.seed0, Hd.seed2, x, normed_seed ? PF_ACT_RELU : PF_ACT_SOFTPLUS);   // fp32 [B,h,w,64]
+  MapF b_prev = mlp_f32(Hd.seed0, Hd.seed2, x, normed_seed ? PF_ACT_RELU : PF_ACT_SOFTPLUS,   // fp32 [B,h,w,64]
+                        "seed_bin_regressor");
   const float* b_t = b_prev.p;
   if (type != PF_BINS_SOFTPLUS) {     // seed centres; normalised to [0, 1] for the normed attractors (zoedepth_v1.py:176-181)
     const long long px = static_cast<long long>(B) * x.H * x.W;
@@ -462,15 +525,18 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
     b_t = sb;
     c.tap_out("seed", sb, 1, px, nb, nb);
   }
-  Map prev_emb = mlp_bf16(Hd.seedproj0, Hd.seedproj2, x);
+  Map prev_emb = mlp_bf16(Hd.seedproj0, Hd.seedproj2, x, "seed_projector");
   const float* centers = nullptr;
   int ph = x.H, pw = x.W;
   for (int i = 0; i < 4; ++i) {
     const Map& xb = x_blocks[i];
-    Map emb = mlp_bf16(Hd.proj0[i], Hd.proj2[i], xb);
+    char mod[16];
+    snprintf(mod, sizeof(mod), "projectors.%d", i);
+    Map emb = mlp_bf16(Hd.proj0[i], Hd.proj2[i], xb, mod);
     Map s = c.map(B, xb.H, xb.W, E);
     if (c.live()) c.chk(pf_add_upsampled(emb.p, B, xb.H, xb.W, E, prev_emb.p, prev_emb.H, prev_emb.W, s.p, c.stream));
-    MapF A = mlp_f32(Hd.att0[i], Hd.att2[i], s, normed_att ? PF_ACT_RELU : PF_ACT_SOFTPLUS);
+    snprintf(mod, sizeof(mod), "attractors.%d", i);
+    MapF A = mlp_f32(Hd.att0[i], Hd.att2[i], s, normed_att ? PF_ACT_RELU : PF_ACT_SOFTPLUS, mod);
     const size_t bytes = static_cast<size_t>(B) * xb.H * xb.W * nb * 4;
     float* b_new = static_cast<float*>(c.alloc(bytes));
     if (normed_att) {
@@ -496,6 +562,7 @@ static void metric_head(Ctx& c, const pf_head& Hd, const Map& x, const Map* x_bl
   Map emb_up = resize(c, prev_emb, H, W);
   float* pt = nullptr;
   GemmOpt g; g.act = PF_ACT_GELU; g.tail = true; g.act2 = PF_ACT_SOFTPLUS; g.out3_ld = 8; g.skip_main = true;
+  c.name("head.clb.0");
   if (rel != nullptr) {
     Map relb = c.map(B, H, W, 1);
     if (c.live()) c.chk(pf_f32_to_bf16(rel->p, static_cast<int64_t>(B) * H * W * rel->ld, relb.p, c.stream));
@@ -523,6 +590,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
   bf16* a0 = static_cast<bf16*>(c.alloc(static_cast<size_t>(B) * npatch * 592 * 2));
   if (c.live()) c.chk(pf_patch_im2col(images, B, H, W, a0, 592, c.stream));
   float* patch = static_cast<float*>(c.alloc(static_cast<size_t>(B) * npatch * D * 4));
+  c.name("patch");
   linear(c, Wb.patch, a0, static_cast<long long>(B) * npatch, 592, 592, patch, 1, D);
   float* x = static_cast<float*>(c.alloc(static_cast<size_t>(rows) * D * 4));
   if (c.live()) c.chk(pf_assemble_tokens(patch, Wb.cls, Wb.pos, B, npatch, D, x, c.stream));
@@ -575,6 +643,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
         c.tap_out(nm, vt, 0, static_cast<long long>(B) * D, seq_pad, seq_pad);
       }
       if (c.live()) c.chk(pf_attention(qk, 2 * D, vt, B, seq, seq_pad, Wb.heads, 0.125f, att, D, c.stream));
+      c.name("b%d.proj", i);
       linear(c, bw.proj, att, rows, D, D, x, 1, D, o1);
       if (c.live())
         c.chk(pf_layernorm_e4m3(x, D, bw.n2w, bw.n2b, 1e-6f, static_cast<int32_t>(rows), D, static_ratio(*bw.fc1.a_amax), h8,
@@ -600,19 +669,23 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
         snprintf(nm, sizeof(nm), "amaxv.%d.qkv", i);
         c.tap_out(nm, hbuf, 0, rows, D, D);
       }
+      c.name("b%d.qkv", i);
       linear(c, bw.qkv, hbuf, rows, D, D, qk, 0, 2 * D, oq);
       if (c.live()) c.chk(pf_attention(qk, 2 * D, vt, B, seq, seq_pad, Wb.heads, 0.125f, att, D, c.stream));
+      c.name("b%d.proj", i);
       linear(c, bw.proj, att, rows, D, D, x, 1, D, o1);
       if (c.live()) c.chk(pf_layernorm(x, D, bw.n2w, bw.n2b, 1e-6f, static_cast<int32_t>(rows), D, hbuf, D, c.stream));
       if (c.tap != nullptr) {
         snprintf(nm, sizeof(nm), "amaxv.%d.fc1", i);
         c.tap_out(nm, hbuf, 0, rows, D, D);
       }
+      c.name("b%d.fc1", i);
       linear(c, bw.fc1, hbuf, rows, D, D, hid, 0, 4 * D, of);
       if (c.tap != nullptr) {
         snprintf(nm, sizeof(nm), "amaxv.%d.fc2", i);
         c.tap_out(nm, hid, 0, rows, 4 * D, 4 * D);
       }
+      c.name("b%d.fc2", i);
       linear(c, bw.fc2, hid, rows, 4 * D, 4 * D, x, 1, D, o2);
     }
     snprintf(nm, sizeof(nm), "block%d", i);
@@ -630,11 +703,13 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
   Map lay[4];
   for (int i = 0; i < 4; ++i) {
     Map p = c.map(B, gh, gw, oc[i]);
+    c.name("proj%d", i);
     linear(c, Wb.proj[i], feats[i].p, feats[i].rows(), D, feats[i].ld, p.p, 0, p.ld);
     if (i == 0 || i == 1) {
       const int k = i == 0 ? 4 : 2;
       Map o = c.map(B, gh * k, gw * k, oc[i]);
       GemmOpt g; g.ps_B = B; g.ps_H = gh; g.ps_W = gw;
+      c.name("rs%d", i);
       linear(c, i == 0 ? Wb.rs0 : Wb.rs1, p.p, p.rows(), oc[i], p.ld, o.p, 0, o.ld, g);
       lay[i] = o;
     } else if (i == 2) {
@@ -644,6 +719,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
       bf16* col = static_cast<bf16*>(c.alloc(static_cast<size_t>(B) * oh * ow * 9 * oc[3] * 2));
       if (c.live()) c.chk(pf_im2col_3x3_s2(p.p, B, gh, gw, oc[3], p.ld, col, c.stream));
       Map o = c.map(B, oh, ow, oc[3]);
+      c.name("rs3");
       linear(c, Wb.rs3, col, static_cast<long long>(B) * oh * ow, 9 * oc[3], 9 * oc[3], o.p, 0, o.ld);
       lay[i] = o;
     }
@@ -679,6 +755,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
       amax_tap(kRn[i], lay[i]);
       rn_relu[i] = c.map(lay[i].B, lay[i].H, lay[i].W, C);
       GemmOpt g; g.relu_copy = &rn_relu[i];
+      c.name("rn%d", i);
       rn[i] = conv1(c, Wb.rn[i], lay[i], g);
     }
   }
@@ -689,10 +766,12 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
     snprintf(n2, sizeof(n2), "refinenet%d.resConfUnit%d.conv2", wi, u);
     amax_tap(n1, xrelu);
     GemmOpt g1; g1.act = PF_ACT_RELU;
+    c.name("ff%d.u%d.c1", wi, u);
     Map t = conv1(c, Wb.ff_c1[wi - 1][u - 1], xrelu, g1);
     amax_tap(n2, t);
     GemmOpt g2; g2.res1 = &xin; g2.res2 = extra;
     if (relu_copy) { *relu_copy = c.map(xin.B, xin.H, xin.W, C); g2.relu_copy = relu_copy; }
+    c.name("ff%d.u%d.c2", wi, u);
     return conv1(c, Wb.ff_c2[wi - 1][u - 1], t, g2);
   };
   // the same unit in FP8: x8 is the e4m3 ReLU copy of xin at conv1's ratio; copy8 (when given) receives y's e4m3 ReLU
@@ -723,6 +802,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
       if (path != nullptr) s = rcu(wi, 1, rn[i], rn_relu[i], path, &s_relu);
       y = rcu(wi, 2, s, s_relu, nullptr, nullptr);
     }
+    c.name("ff%d.out", wi);
     y = conv1(c, Wb.ff_out[wi - 1], y);
     return resize(c, y, OH, OW);
   };
@@ -740,6 +820,7 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
                   nullptr, 0, nullptr);
   } else {
     amax_tap("output_conv1", p1);
+    c.name("oc1");
     o = conv1(c, Wb.oc1, p1);
   }
   o = resize(c, o, H, W);
@@ -750,7 +831,9 @@ static void branch_run(Ctx& c, const pf_branch& Wb, const float* images, int B, 
   }
   // output_conv2: 3x3 C/2 -> 32 + ReLU (the hooked `out_conv` tap) with the 1x1 32 -> 1 + ReLU fused in its epilogue
   GemmOpt go; go.act = PF_ACT_RELU; go.tail = true; go.act2 = PF_ACT_RELU; go.out3 = rel.p; go.out3_ld = rel.ld;
+  c.name("oc2.0");
   Map out_conv = conv1(c, Wb.oc2, o, go);
+  c.name("conv2");
   Map x_d0 = conv1(c, Wb.conv2, rn[3]);
   c.tap_out("rel", rel.p, 1, static_cast<long long>(B) * H * W, 1, 8);
   float* depth = static_cast<float*>(c.alloc(static_cast<size_t>(B) * H * W * 4));
@@ -790,14 +873,18 @@ static void g2l_run(Ctx& c, const pf_fusion& Wf, const pf_map* coarse, pf_map* o
       const pf_g2l_block& bw = L.blocks[b];
       const int shift = (b % 2 == 0) ? 0 : WS / 2;
       if (c.live()) c.chk(pf_swin_norm_pad_batched(x, bw.n1w, bw.n1b, 1e-5f, B, h, w, Hp, Wp, cc, npad, c.stream));
+      c.name("g2l%d.b%d.qkv", i, b);
       linear(c, bw.qkv, npad, prow, cc, cc, qkv, 0, 3 * cc);
       if (c.live()) c.chk(pf_window_attention_batched(qkv, bw.table, B, Hp, Wp, cc, L.heads, shift, att, c.stream));
+      c.name("g2l%d.b%d.proj", i, b);
       linear(c, bw.proj, att, prow, cc, cc, prj, 1, cc);
       if (c.live()) c.chk(pf_swin_residual_crop_batched(x, prj, B, h, w, Hp, Wp, cc, c.stream));
       if (c.live()) c.chk(pf_layernorm(x, cc, bw.n2w, bw.n2b, 1e-5f, static_cast<int32_t>(rows), cc, hb, cc, c.stream));
       GemmOpt g1; g1.act = PF_ACT_GELU;
+      c.name("g2l%d.b%d.fc1", i, b);
       linear(c, bw.fc1, hb, rows, cc, cc, hid, 0, 4 * cc, g1);
       GemmOpt g2; g2.gamma = L.ones;
+      c.name("g2l%d.b%d.fc2", i, b);
       linear(c, bw.fc2, hid, rows, 4 * cc, 4 * cc, x, 1, cc, g2);
     }
     Map o = c.map(B, h, w, cc);
@@ -822,6 +909,7 @@ static void fusion_run(Ctx& c, const pf_fusion& Wf, const float* crops, const fl
       c.chk(pf_roi_crop_zoom_batched(cf.p, 0, cf.H, cf.W, pad_to(cf.C, 8), cf.ld, tile_image, boxes, T,
                                      static_cast<float>(cf.H) / H, roi.p, roi.ld, 0, c.stream));
     const Map* a[2] = {&roi, &ff};
+    c.name("fc%d", i);
     guide[i] = conv(c, Wf.fc[i], a, 2);
   }
   float* droi = static_cast<float*>(c.alloc(static_cast<size_t>(T) * H * W * 4));
@@ -906,10 +994,11 @@ size_t pf_g2l_workspace_bytes(const pf_fusion* w, const pf_map* coarse_feats) {
   return c.off + 256;
 }
 
-int pf_g2l_forward(const pf_fusion* w, const pf_map* coarse_feats, void* ws, size_t ws_bytes, pf_map* out, void* stream) {
+int pf_g2l_forward(const pf_fusion* w, const pf_map* coarse_feats, void* ws, size_t ws_bytes, pf_map* out, pf_tap_fn tap,
+                   void* tap_user, void* stream) {
   if (!w || !coarse_feats || !ws || !out) return set_error("pf_g2l_forward: null argument");
   if (reinterpret_cast<uintptr_t>(ws) & 255) return set_error("pf_g2l_forward: workspace must be 256-byte aligned");
-  Ctx c = make_ctx(ws, ws_bytes, false, stream, nullptr, nullptr);
+  Ctx c = make_ctx(ws, ws_bytes, false, stream, tap, tap_user);
   g2l_run(c, *w, coarse_feats, out);
   return c.err;
 }

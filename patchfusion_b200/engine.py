@@ -482,12 +482,16 @@ class Engine:
     def _maps(self, arena, pf_maps):
         return [Map(self._view(arena, m.ptr, (m.B, m.H, m.W, m.ld), BF16), m.C) for m in pf_maps]
 
-    def _tap_cb(self, arena, taps):
+    def _tap_cb(self, arena, taps, inputs=()):
+        """inputs: the Maps of the call's inputs outside `arena` that a layer tap may name (a conv's source)"""
+        spans = [arena] + [m.t.reshape(-1).view(torch.uint8) for m in inputs]
+
         def cb(user, name, ptr, is_f32, rows, cols, ld):
             # is_f32: 0 bf16, 1 fp32, 2 e4m3 bytes (the static FP8 convs' operand maps)
             if name.startswith(b'amaxv.') or name.startswith(b'amaxd.'):
                 return      # the bf16 branch's calibration inputs (_calib_vit_cb): not kept
-            t = self._view(arena, ptr, (rows, ld), (BF16, F32, torch.uint8)[is_f32])
+            span = next(s_ for s_ in spans if 0 <= ptr - s_.data_ptr() < s_.numel())
+            t = self._view(span, ptr, (rows, ld), (BF16, F32, torch.uint8)[is_f32])
             taps[name.decode()] = t[:, :cols].clone()
         return cb
 
@@ -565,14 +569,15 @@ class Engine:
             arr[i].B, arr[i].H, arr[i].W = m.t.shape[0], m.t.shape[1], m.t.shape[2]
         return arr
 
-    def g2l(self, coarse_feats):
+    def g2l(self, coarse_feats, taps=None):
         """The six tile-invariant G2L maps of the whole-image coarse taps (computed once per image).  The maps may hold
         a batch of B images: one call then computes the B images' maps, batch B out."""
         from . import stage
         cm = self._pf_maps(coarse_feats)
         need = stage.g2l_workspace_bytes(self.c_fusion, cm)
         arena = self.arena('g2l', need)
-        out = stage.g2l_forward(self.c_fusion, cm, arena.data_ptr(), need)
+        tap = self._tap_cb(arena, taps) if taps is not None else None
+        out = stage.g2l_forward(self.c_fusion, cm, arena.data_ptr(), need, tap)
         return self._maps(arena, out)
 
     def fusion_bytes(self, T, g2l_maps):
@@ -602,7 +607,7 @@ class Engine:
             assert t_.dtype == F32 and t_.is_contiguous()
         if tile_image is not None:
             assert tile_image.dtype == torch.int32 and tile_image.is_contiguous() and tile_image.numel() == T
-        tap = self._tap_cb(arena, taps) if taps is not None else None
+        tap = self._tap_cb(arena, taps, fine_feats) if taps is not None else None
         if tap is None and self.calib is not None:
             tap = self._calib_cb(arena)
         stage.fusion_forward(cfu, crops, boxes, T, fine_depth, self._pf_maps(fine_feats), coarse_depth,

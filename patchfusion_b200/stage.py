@@ -82,7 +82,7 @@ def _bind():
     h.pf_branch_forward.restype = C.c_int
     h.pf_branch_forward.argtypes = [C.POINTER(PfBranch), vp, i32, vp, C.c_size_t, C.POINTER(PfBranchOut), vp, vp, vp]
     h.pf_g2l_forward.restype = C.c_int
-    h.pf_g2l_forward.argtypes = [C.POINTER(PfFusion), C.POINTER(PfMap), vp, C.c_size_t, C.POINTER(PfMap), vp]
+    h.pf_g2l_forward.argtypes = [C.POINTER(PfFusion), C.POINTER(PfMap), vp, C.c_size_t, C.POINTER(PfMap), vp, vp, vp]
     h.pf_fusion_forward.restype = C.c_int
     h.pf_fusion_forward.argtypes = [C.POINTER(PfFusion), vp, vp, i32, vp, C.POINTER(PfMap), vp, C.POINTER(PfMap),
                                     C.POINTER(PfMap), vp, C.c_size_t, vp, vp, vp, vp]
@@ -148,9 +148,11 @@ def branch_forward(cb, images, B, ws_ptr, ws_bytes, tap=None):
     return out
 
 
-def g2l_forward(cf, maps, ws_ptr, ws_bytes):
+def g2l_forward(cf, maps, ws_ptr, ws_bytes, tap=None):
     out = (PfMap * 6)()
-    rc = _bind().pf_g2l_forward(C.byref(cf), maps, ws_ptr, ws_bytes, out, lib.stream_ptr())
+    cbk = TAP_FN(tap) if tap is not None else None
+    rc = _bind().pf_g2l_forward(C.byref(cf), maps, ws_ptr, ws_bytes, out, C.cast(cbk, vp) if cbk is not None else None,
+                                None, lib.stream_ptr())
     _check(rc, 'pf_g2l_forward')
     return out
 
